@@ -1,5 +1,5 @@
 // K1: explicit leapfrog, dense shared metric, fused target gradient, n_steps per launch --
-// FP64 tensor-core kernel (DMMA m8n8k4) for dim <= 128.
+// FP64 tensor-core kernel (DMMA m16n8k16, m8n8k4 for lone row tiles) for dim <= 128.
 //
 // Replaces, for every chain at once (reference paths):
 //   LeapfrogIntegrator._step          integrators.py:170-173
@@ -10,7 +10,9 @@
 // The one genuine contraction on the path is V = P * A  ([chains x D] . [D x D], A = M^-1
 // explicit and symmetric): 2 D^2 flop per chain-step against 32 D bytes of state, i.e. above the
 // H100 fp64 ridge (67 TFLOP/s on the tensor cores against 3.35 TB/s, data sheet), so the kernel
-// is organised around the FP64 tensor pipe (DMMA.8x8x4, mma.sync m8n8k4 f64 on sm_90a).
+// is organised around the FP64 tensor pipe.  On sm_90a the m16n8k{4,8,16} f64 shapes issue at
+// 256 flop/clk/SM, m8n8k4 at half that (profiles/tools/fp64_peak.cu): a group that owns two row
+// tiles contracts them as the 16 rows of DMMA.16x8x16; a lone tile uses DMMA.8x8x4.
 //
 // Work decomposition (one CTA per SM, 16 warps, 4 groups x 4 warps):
 //   * a CTA owns up to 64 chains = 8 row tiles of 8 chains; every group takes two tiles --
@@ -39,6 +41,17 @@ __device__ __forceinline__ void dmma_m8n8k4(double& c0, double& c1, double a, do
       "mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};\n"
       : "+d"(c0), "+d"(c1)
       : "d"(a), "d"(b));
+}
+
+__device__ __forceinline__ void dmma_m16n8k16(double& c0, double& c1, double& c2, double& c3,
+                                              const double2 (&a)[2][2], const double2 (&b)[2]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, "
+      "{%4,%5,%6,%7,%8,%9,%10,%11}, {%12,%13,%14,%15}, {%0,%1,%2,%3};\n"
+      : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3)
+      : "d"(a[0][0].x), "d"(a[1][0].x), "d"(a[0][0].y), "d"(a[1][0].y),
+        "d"(a[0][1].x), "d"(a[1][1].x), "d"(a[0][1].y), "d"(a[1][1].y),
+        "d"(b[0].x), "d"(b[0].y), "d"(b[1].x), "d"(b[1].y));
 }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
@@ -103,14 +116,15 @@ struct DmmaSmem {
 // never leave the accumulator registers.
 //
 // Scheduling facts this is written around (profiles/tools fp64_arb / fp64_mix / k1_bench -DK1_TRACE):
-// a warp whose next instruction is a scalar FP64 operation makes NO progress while two or more
-// other warps of its SM sub-partition stream DMMAs, so the per-step update phase of every group
-// ends up running after the drifts of the whole sub-partition (the groups lock-step) and the
-// step time is  drift (DMMA-pipe bound) + update phase (issue / latency bound).  The update phase
-// is therefore kept as short as possible: no bounds logic (phantom coordinates are zero and stay
-// zero under every registry target's kick), one FMA chain for the reduction, the per-chain scalar
-// (funnel: exp(-v)) published by its owner instead of being summed, own momenta pre-loaded
-// before the group barrier, two barriers per step.
+// a warp whose next instruction is a scalar FP64 operation makes almost NO progress while other
+// warps of its SM sub-partition stream DMMAs (two or more streaming DMMA.8x8x4; a single one
+// streaming DMMA.16x8x16 already holds it to ~390 cycles per instruction), so the per-step
+// update phase of every group ends up running after the drifts of the whole sub-partition (the
+// groups lock-step) and the step time is  drift (DMMA-pipe bound) + update phase (issue /
+// latency bound).  The update phase is therefore kept as short as possible: no bounds logic
+// (phantom coordinates are zero and stay zero under every registry target's kick), one FMA chain
+// for the reduction, the per-chain scalar (funnel: exp(-v)) published by its owner instead of
+// being summed, own momenta pre-loaded before the group barrier, two barriers per step.
 //
 // PC = true: per-chain step sizes (adaptive warm-up, adapters.py:40-235 per chain).  sm.A then holds
 // A unscaled (step_size = 1) and the momentum tile holds  s = eps_c * dir * p:
@@ -135,23 +149,29 @@ __device__ __forceinline__ void leapfrog_dmma_group(
 
   // registers: positions of the slice in C-fragment layout (row 8mt + r, columns
   // col0 + 8nt + 2c + {0,1}); signed momenta live in sm.P with the same ownership
-  double q[MT][NT][2], sgn[MT], mhr[PC ? MT : 1];
+  double q[MT][NT][2], mhr[PC ? MT : 1];
   bool live[MT];
-  double2* pslot[MT];  // &sm.P[row][col0 + 2c]; + 4*nt double2 per column tile
   int row[MT];
+  // momentum scale of a live chain: dir (+-1), times eps_c with per-chain step sizes; read again
+  // for the store rather than held in registers through the launch
+  auto load_scale = [&](int64_t ch) {
+    const double d = (dir != nullptr && dir[ch] < 0) ? -1.0 : 1.0;
+    return PC ? d * step_sizes[ch] : d;
+  };
+  // own momentum slots &sm.P[row[mt]][col0 + 8nt + 2c], addressed from one 32-bit offset (the
+  // MT x NT slots fold into load / store immediates; pointers would hold 2 registers per tile)
+  const uint32_t pofs = (uint32_t)((row0 + r) * LDA + col0 + 2 * c);
+  auto pslot = [&](int mt, int nt) -> double2& {
+    return *reinterpret_cast<double2*>(&sm.P[pofs + mt * 8 * LDA + 8 * nt]);
+  };
 
 #pragma unroll
   for (int mt = 0; mt < MT; ++mt) {
     row[mt] = row0 + 8 * mt + r;
     const int64_t ch = chain0 + row[mt];
     live[mt] = ch < n_chains;
-    sgn[mt] = (live[mt] && dir != nullptr && dir[ch] < 0) ? -1.0 : 1.0;
-    if (PC) {  // sgn becomes the load scale dir * eps_c
-      const double e = live[mt] ? step_sizes[ch] : 0.0;
-      sgn[mt] *= e;
-      mhr[mt] = -0.5 * (e * e);
-    }
-    pslot[mt] = reinterpret_cast<double2*>(&sm.P[row[mt] * LDA + col0 + 2 * c]);
+    const double sgn = live[mt] ? load_scale(ch) : (PC ? 0.0 : 1.0);
+    if (PC) mhr[mt] = -0.5 * (sgn * sgn);
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
       const int i = col0 + 8 * nt + 2 * c;
@@ -166,7 +186,7 @@ __device__ __forceinline__ void leapfrog_dmma_group(
         }
       }
       q[mt][nt][0] = a.x, q[mt][nt][1] = a.y;
-      pslot[mt][4 * nt] = make_double2(sgn[mt] * b.x, sgn[mt] * b.y);
+      pslot(mt, nt) = make_double2(sgn * b.x, sgn * b.y);
     }
   }
 
@@ -209,7 +229,7 @@ __device__ __forceinline__ void leapfrog_dmma_group(
 #pragma unroll
       for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
-        for (int nt = 0; nt < NT; ++nt) pv[mt][nt] = pslot[mt][4 * nt];  // own slots: no hazard
+        for (int nt = 0; nt < NT; ++nt) pv[mt][nt] = pslot(mt, nt);  // own slots: no hazard
     }
     MB200_K1_TRACE(2);
     named_barrier_sync(bar_id, 128);
@@ -241,7 +261,7 @@ __device__ __forceinline__ void leapfrog_dmma_group(
           for (int k = 0; k < KICKS; ++k)
             target.kick_pair_nl(mhm, q[mt][nt][0], q[mt][nt][1], v.x, v.y);
         }
-        pslot[mt][4 * nt] = v;
+        pslot(mt, nt) = v;
       }
     }
     MB200_K1_TRACE(4);
@@ -253,43 +273,67 @@ __device__ __forceinline__ void leapfrog_dmma_group(
   using K2 = std::integral_constant<int, 2>;
 
   // acc += S * (eps A) on the tensor pipe (acc = q for the drift, acc = 0 for the energy).
-  // Fragments are fetched with 128-bit loads: lane c of a row holds k = 8J + 2c and 8J + 2c + 1,
-  // the two DMMAs of a k-pair contract {8J, 8J+2, 8J+4, 8J+6} and {8J+1, ..., 8J+7} (the pairing of
-  // lanes with k is free as long as the A and B fragments agree).
+  // Fragments are fetched with 128-bit loads: lane c of a row holds k = 8J + 2c and 8J + 2c + 1.
+  // The pairing of lanes with k is free as long as the A and B fragments agree.
   auto drift = [&](double (&acc)[MT][NT][2]) {
     const double2* a_base = reinterpret_cast<const double2*>(&sm.P[(row0 + r) * LDA + 2 * c]);
     const double2* b_base = reinterpret_cast<const double2*>(&sm.A[(col0 + r) * LDA + 2 * c]);
-    // a single row tile gives a warp only NT independent accumulator chains (DMMA latency ~ 10
-    // issue slots): the two halves of every k-pair then go to separate accumulator sets that are
-    // added at the end (same products, summed in a different order)
-    constexpr bool KSPLIT = (MT == 1);
-    double acc2[KSPLIT ? NT : 1][2];
-    if (KSPLIT) {
+    if constexpr (MT == 2) {
+      // The group's two row tiles are the 16 rows of DMMA.16x8x16 (twice the FP64 rate of
+      // DMMA.8x8x4 on sm_90): rows r / r + 8 are the C fragment's c0,c1 / c2,c3, i.e. q[0][nt]
+      // and q[1][nt].  Fragment slot i (logical k = c + 4i) of lane c holds physical k
+      // 16J + {2c, 2c + 1, 8 + 2c, 9 + 2c}[i]: the two 128-bit loads of k-pairs 2J and 2J + 1.
+#pragma unroll 2
+      for (int j = 0; j < KS / 4; ++j) {
+        double2 a[2][2], b[NT][2];
 #pragma unroll
-      for (int nt = 0; nt < NT; ++nt) acc2[nt][0] = 0.0, acc2[nt][1] = 0.0;
-    }
+        for (int mt = 0; mt < 2; ++mt)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) a[mt][h] = a_base[mt * 4 * LDA + 4 * (2 * j + h)];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) b[nt][h] = b_base[nt * 4 * LDA + 4 * (2 * j + h)];
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt)
+          dmma_m16n8k16(acc[0][nt][0], acc[0][nt][1], acc[1][nt][0], acc[1][nt][1], a, b[nt]);
+      }
+    } else {
+      // DMMA.8x8x4 per row tile: the two DMMAs of a k-pair contract {8J, 8J+2, 8J+4, 8J+6} and
+      // {8J+1, ..., 8J+7}.  A single row tile gives a warp only NT independent accumulator
+      // chains (DMMA latency ~ 10 issue slots): the two halves of every k-pair then go to
+      // separate accumulator sets that are added at the end (same products, summed in a
+      // different order)
+      constexpr bool KSPLIT = (MT == 1);
+      double acc2[KSPLIT ? NT : 1][2];
+      if (KSPLIT) {
+#pragma unroll
+        for (int nt = 0; nt < NT; ++nt) acc2[nt][0] = 0.0, acc2[nt][1] = 0.0;
+      }
 #pragma unroll 4
-    for (int j = 0; j < KS / 2; ++j) {
-      double2 a[MT], b[NT];
+      for (int j = 0; j < KS / 2; ++j) {
+        double2 a[MT], b[NT];
 #pragma unroll
-      for (int mt = 0; mt < MT; ++mt) a[mt] = a_base[mt * 4 * LDA + 4 * j];
+        for (int mt = 0; mt < MT; ++mt) a[mt] = a_base[mt * 4 * LDA + 4 * j];
 #pragma unroll
-      for (int nt = 0; nt < NT; ++nt) b[nt] = b_base[nt * 4 * LDA + 4 * j];
+        for (int nt = 0; nt < NT; ++nt) b[nt] = b_base[nt * 4 * LDA + 4 * j];
 #pragma unroll
-      for (int mt = 0; mt < MT; ++mt)
+        for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
-        for (int nt = 0; nt < NT; ++nt) dmma_m8n8k4(acc[mt][nt][0], acc[mt][nt][1], a[mt].x, b[nt].x);
+          for (int nt = 0; nt < NT; ++nt)
+            dmma_m8n8k4(acc[mt][nt][0], acc[mt][nt][1], a[mt].x, b[nt].x);
 #pragma unroll
-      for (int mt = 0; mt < MT; ++mt)
+        for (int mt = 0; mt < MT; ++mt)
 #pragma unroll
-        for (int nt = 0; nt < NT; ++nt) {
-          if (KSPLIT) dmma_m8n8k4(acc2[nt][0], acc2[nt][1], a[mt].y, b[nt].y);
-          else dmma_m8n8k4(acc[mt][nt][0], acc[mt][nt][1], a[mt].y, b[nt].y);
-        }
-    }
-    if (KSPLIT) {
+          for (int nt = 0; nt < NT; ++nt) {
+            if (KSPLIT) dmma_m8n8k4(acc2[nt][0], acc2[nt][1], a[mt].y, b[nt].y);
+            else dmma_m8n8k4(acc[mt][nt][0], acc[mt][nt][1], a[mt].y, b[nt].y);
+          }
+      }
+      if (KSPLIT) {
 #pragma unroll
-      for (int nt = 0; nt < NT; ++nt) acc[0][nt][0] += acc2[nt][0], acc[0][nt][1] += acc2[nt][1];
+        for (int nt = 0; nt < NT; ++nt) acc[0][nt][0] += acc2[nt][0], acc[0][nt][1] += acc2[nt][1];
+      }
     }
   };
 
@@ -317,16 +361,17 @@ __device__ __forceinline__ void leapfrog_dmma_group(
   for (int mt = 0; mt < MT; ++mt) {
     const int64_t ch = chain0 + row[mt];
     if (!live[mt]) continue;
+    const double sgn = load_scale(ch);
 #pragma unroll
     for (int nt = 0; nt < NT; ++nt) {
       const int i = col0 + 8 * nt + 2 * c;
       if (i < dim) {
-        const double2 sv = pslot[mt][4 * nt];
-        double2 pv = make_double2(sgn[mt] * sv.x, sgn[mt] * sv.y);  // dir = +-1: exact
+        const double2 sv = pslot(mt, nt);
+        double2 pv = make_double2(sgn * sv.x, sgn * sv.y);  // dir = +-1: exact
         if (PC) {
           // s = (dir eps_c) p  ->  p = s / (dir eps_c); a chain with eps_c = 0 has not moved
-          if (sgn[mt] != 0.0) {
-            pv = make_double2(sv.x / sgn[mt], sv.y / sgn[mt]);
+          if (sgn != 0.0) {
+            pv = make_double2(sv.x / sgn, sv.y / sgn);
           } else {
             pv.x = p_in[(size_t)ch * dim + i];
             pv.y = (i + 1 < dim) ? p_in[(size_t)ch * dim + i + 1] : 0.0;
@@ -377,7 +422,7 @@ __device__ __forceinline__ void leapfrog_dmma_group(
       kin[mt] = 0.0;
 #pragma unroll
       for (int nt = 0; nt < NT; ++nt) {
-        const double2 sv = pslot[mt][4 * nt];
+        const double2 sv = pslot(mt, nt);
         kin[mt] = fma(sv.x, u[mt][nt][0], kin[mt]);
         kin[mt] = fma(sv.y, u[mt][nt][1], kin[mt]);
       }
