@@ -13,6 +13,13 @@
  *    copied by value into the launch).
  *  - `dir` may be NULL (all chains +1) or int32[n_chains] with entries +-1; the signed time
  *    step of a chain is `dir * step_size` (integrators.py:79).
+ *  - Integrator entry points take `double step_size, const double* step_sizes, int32_t n_steps,
+ *    const int32_t* n_steps_per_chain`.  `step_sizes` is NULL or a device array [n_chains]: when
+ *    given, chain c uses step_sizes[c] instead of step_size (during warm-up every chain carries
+ *    its own dual-averaging step size: adapters.py:262-283, 373; the initial coarse search halves
+ *    / doubles it chain by chain: adapters.py:285-343).  `n_steps_per_chain` is NULL or a device
+ *    array [n_chains]: when given, chain c takes min(n_steps_per_chain[c], n_steps) steps
+ *    (MetropolisRandomIntegrationTransition, transitions.py:355-412).
  *  - Out-of-place: `*_out` may alias `*_in` (in-place) or be distinct buffers, so that
  *    `Integrator.step` keeps its "returns a new state, argument untouched" contract
  *    (integrators.py:78-80, tests/test_integrators.py:110-124) without an extra copy.
@@ -35,7 +42,7 @@
 extern "C" {
 #endif
 
-#define MB200_VERSION 100
+#define MB200_VERSION 101
 
 /* per-chain status codes */
 #define MB200_STATUS_OK 0
@@ -124,22 +131,39 @@ int mb200_set_call_counters(int32_t* counters);
  *           System.h1_flow/dh1_dpos/grad_neg_log_dens (systems.py:109-152) +
  *           EuclideanMetricSystem.h2_flow/dh2_dmom (systems.py:352-363) +
  *           explicit-inverse matvec (matrices.py:222-226, 1183-1188).
+ * "Next" row N4: symmetric composition (splitting) integrators --
+ * SymmetricCompositionIntegrator and the BCSS 2/3/4-stage schemes (integrators.py:176-378):
+ *   coefficients  NULL: the leapfrog schedule {0.5, 1, 0.5} (n_flows / initial_h1_flow_step are
+ *                 ignored).  Else a HOST array of the full symmetric sequence of n_flows (odd)
+ *                 coefficients (integrators.py:268-277): each step applies the alternating flows
+ *                 a, b, a, ..., a over coefficients[i] * dt, a = h1_flow (kick) if
+ *                 initial_h1_flow_step else h2_flow (drift).
  * h_out (optional, [n_chains]): Hamiltonian of the returned state (systems.py:187-196,348-350).
+ * n_done[c] receives the number of steps chain c took.  With a dense metric, the leapfrog
+ * schedule, n_steps_per_chain == NULL and n_steps > 0 it runs on the tensor-core kernel (which
+ * applies per-chain step sizes on the momentum side: tile s = eps_c * dir * p against the
+ * unscaled metric); otherwise on the general-dimension kernel.
  */
 int mb200_leapfrog_euclidean(const double* pos_in, const double* mom_in, double* pos_out,
                              double* mom_out, const int32_t* dir, int64_t n_chains, int32_t dim,
-                             double step_size, int32_t n_steps, int32_t metric_kind,
-                             const double* metric_inv, const mb200_model* model, double* h_out,
-                             int32_t* status, int32_t* n_done, void* stream);
+                             double step_size, const double* step_sizes, int32_t n_steps,
+                             const int32_t* n_steps_per_chain, int32_t n_flows,
+                             const double* coefficients, int32_t initial_h1_flow_step,
+                             int32_t metric_kind, const double* metric_inv,
+                             const mb200_model* model, double* h_out, int32_t* status,
+                             int32_t* n_done, void* stream);
 
 /* Diagnostic: identical contract, but always through the general-dimension kernel (never the
  * tensor-core kernel); used by the tests to cross-check the two implementations. */
 int mb200_leapfrog_euclidean_generic(const double* pos_in, const double* mom_in, double* pos_out,
                                      double* mom_out, const int32_t* dir, int64_t n_chains,
-                                     int32_t dim, double step_size, int32_t n_steps,
-                                     int32_t metric_kind, const double* metric_inv,
-                                     const mb200_model* model, double* h_out, int32_t* status,
-                                     int32_t* n_done, void* stream);
+                                     int32_t dim, double step_size, const double* step_sizes,
+                                     int32_t n_steps, const int32_t* n_steps_per_chain,
+                                     int32_t n_flows, const double* coefficients,
+                                     int32_t initial_h1_flow_step, int32_t metric_kind,
+                                     const double* metric_inv, const mb200_model* model,
+                                     double* h_out, int32_t* status, int32_t* n_done,
+                                     void* stream);
 
 /* Hamiltonian h = l(q) + p.M^-1 p / 2 of a Euclidean-metric system (systems.py:187-196, 348-350). */
 int mb200_hamiltonian_euclidean(const double* pos, const double* mom, int64_t n_chains,
@@ -168,11 +192,12 @@ int mb200_euclidean_eval(const double* pos, const double* mom, int64_t n_chains,
  */
 int mb200_constrained_leapfrog_euclidean(
     const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, int32_t n_steps,
-    int32_t n_inner_step, int32_t metric_kind, const double* metric_inv, const mb200_model* model,
-    int32_t projection_solver, double constraint_tol, double position_tol, double divergence_tol,
-    int32_t max_iters, int32_t max_line_search_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* newton_iters, void* stream);
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream);
 
 /*
  * n_steps implicit generalised-leapfrog steps on a Riemannian-metric system, fixed-point
@@ -188,11 +213,11 @@ int mb200_constrained_leapfrog_euclidean(
  */
 int mb200_implicit_leapfrog_riemannian(
     const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, int32_t n_steps,
-    const mb200_model* model, int32_t fp_solver, double fp_convergence_tol,
-    double fp_divergence_tol, int32_t fp_max_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* fp_iters, void* workspace, int64_t workspace_bytes,
-    void* stream);
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* workspace, int64_t workspace_bytes, void* stream);
 
 int64_t mb200_implicit_workspace_bytes(int64_t n_chains, int32_t dim, const mb200_model* model);
 
@@ -230,22 +255,6 @@ int mb200_selftest_fixed_point(int32_t func_id, int32_t fp_solver, const double*
                                int32_t* iters_out, int32_t* status, void* stream);
 
 /*
- * "Next" row N4: symmetric composition (splitting) integrators on a Euclidean-metric system --
- * SymmetricCompositionIntegrator and the BCSS 2/3/4-stage schemes (integrators.py:176-378):
- * each step applies n_flows (odd) alternating flows a, b, a, ..., a over coefficients[i] * dt,
- * a = h1_flow (kick) if initial_h1_flow_step else h2_flow (drift).  `coefficients` is a HOST
- * array of the full symmetric sequence (integrators.py:268-277).  Same other arguments and
- * conventions as mb200_leapfrog_euclidean (which is the schedule {0.5, 1, 0.5}).
- */
-int mb200_composition_euclidean(const double* pos_in, const double* mom_in, double* pos_out,
-                                double* mom_out, const int32_t* dir, int64_t n_chains,
-                                int32_t dim, double step_size, int32_t n_steps, int32_t n_flows,
-                                const double* coefficients, int32_t initial_h1_flow_step,
-                                int32_t metric_kind, const double* metric_inv,
-                                const mb200_model* model, double* h_out, int32_t* status,
-                                int32_t* n_done, void* stream);
-
-/*
  * Diagnostic: the per-chain symmetric eigensolver (K3, parallel cyclic Jacobi; replaces
  * numpy.linalg.eigh at matrices.py:437, 1658) on arbitrary dense symmetric matrices
  * [n_matrices x dim x dim].  eigvec holds the eigenvectors as columns (row-major), eigval is
@@ -276,10 +285,11 @@ int mb200_selftest_dense_factor(const double* matrices, const double* rhs, int64
  */
 int mb200_implicit_midpoint_riemannian(
     const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, int32_t n_steps,
-    const mb200_model* model, int32_t fp_solver, double fp_convergence_tol,
-    double fp_divergence_tol, int32_t fp_max_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* fp_iters, void* stream);
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* stream);
 
 /*
  * Momentum refresh for the non-Euclidean systems (row N1).
@@ -308,33 +318,6 @@ int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_o
                              int32_t* status, void* stream);
 
 /*
- * "Next" row N3 (and the random-length transition of N1): explicit leapfrog / symmetric
- * composition with PER-CHAIN step sizes and, optionally, per-chain trajectory lengths.
- *   step_sizes         [n_chains] device array -- during warm-up every chain carries its own
- *                      dual-averaging step size (adapters.py:262-283, 373); the initial coarse
- *                      search halves / doubles it chain by chain (adapters.py:285-343)
- *   n_steps_per_chain  [n_chains] device array or NULL; chain c takes
- *                      min(n_steps_per_chain[c], max_n_steps) steps
- *                      (MetropolisRandomIntegrationTransition, transitions.py:355-412)
- *   coefficients       HOST array of n_flows composition coefficients or NULL for the leapfrog
- *                      schedule {0.5, 1, 0.5} (then n_flows / initial_h1_flow_step are ignored)
- * n_done[c] receives the number of steps chain c took.  Other arguments as
- * mb200_leapfrog_euclidean.  With a dense metric, the leapfrog schedule and one trajectory
- * length (n_steps_per_chain == NULL) it runs on the tensor-core kernel, which then applies the
- * step size on the momentum side (tile s = eps_c * dir * p against the unscaled metric);
- * otherwise on the general-dimension kernel.
- */
-int mb200_leapfrog_euclidean_per_chain(const double* pos_in, const double* mom_in, double* pos_out,
-                                       double* mom_out, const int32_t* dir, int64_t n_chains,
-                                       int32_t dim, const double* step_sizes,
-                                       const int32_t* n_steps_per_chain, int32_t max_n_steps,
-                                       int32_t n_flows, const double* coefficients,
-                                       int32_t initial_h1_flow_step, int32_t metric_kind,
-                                       const double* metric_inv, const mb200_model* model,
-                                       double* h_out, int32_t* status, int32_t* n_done,
-                                       void* stream);
-
-/*
  * "Next" row N4: GaussianEuclideanMetricSystem (systems.py:369-474) -- the target density is
  * given relative to the standard Gaussian measure, h1 = l(q), h2 = q.q/2 + p.M^-1 p/2 and
  * h2_flow is the exact rotation of (q, p) in the eigenbasis of M (systems.py:464-474).  Leapfrog
@@ -355,30 +338,6 @@ int mb200_leapfrog_gaussian_euclidean(const double* pos_in, const double* mom_in
                                       const double* metric_inv, const double* rotation,
                                       const mb200_model* model, double* h_out, int32_t* status,
                                       int32_t* n_done, void* stream);
-
-/*
- * Per-chain step sizes / trajectory lengths for the constrained and the implicit integrators
- * (row N3: adapters drive one step size per chain during warm-up, adapters.py:262-283, 373; the
- * coarse initial search relies on per-chain failures, adapters.py:338-340).  Arguments as the
- * scalar entry points with `step_size` replaced by the device array `step_sizes[n_chains]` and
- * `n_steps` by `max_n_steps` plus the optional device array `n_steps_per_chain[n_chains]`
- * (NULL: every chain takes max_n_steps).  `midpoint` != 0 selects ImplicitMidpointIntegrator.
- */
-int mb200_constrained_leapfrog_euclidean_per_chain(
-    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, const double* step_sizes,
-    const int32_t* n_steps_per_chain, int32_t max_n_steps, int32_t n_inner_step,
-    int32_t metric_kind, const double* metric_inv, const mb200_model* model,
-    int32_t projection_solver, double constraint_tol, double position_tol, double divergence_tol,
-    int32_t max_iters, int32_t max_line_search_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* newton_iters, void* stream);
-int mb200_implicit_riemannian_per_chain(
-    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, const double* step_sizes,
-    const int32_t* n_steps_per_chain, int32_t max_n_steps, int32_t midpoint,
-    const mb200_model* model, int32_t fp_solver, double fp_convergence_tol,
-    double fp_divergence_tol, int32_t fp_max_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* fp_iters, void* stream);
 
 /*
  * "Next" row N4: dynamic-length HMC transitions (NUTS) on a Euclidean-metric system with the

@@ -58,29 +58,27 @@ _I64, _I32, _F64, _P = ctypes.c_int64, ctypes.c_int32, ctypes.c_double, ctypes.c
 _MP = ctypes.POINTER(Model)
 _NP = ctypes.POINTER(NutsOptions)
 
+# mb200_leapfrog_euclidean and its general-kernel twin
+_LEAPFROG_EUCLIDEAN_ARGS = [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _P, _I32, _I32,
+                            _P, _MP, _P, _P, _P, _P]
+
 # symbol -> (restype, argtypes): every symbol declared in include/mici_b200.h
 SIGNATURES = {
     "mb200_version": (ctypes.c_int, []),
     "mb200_last_error": (ctypes.c_char_p, []),
     "mb200_set_call_counters": (ctypes.c_int, [_P]),
-    "mb200_leapfrog_euclidean": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _I32, _I32, _P, _MP, _P, _P, _P, _P],
-    ),
-    "mb200_leapfrog_euclidean_generic": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _I32, _I32, _P, _MP, _P, _P, _P, _P],
-    ),
+    "mb200_leapfrog_euclidean": (ctypes.c_int, _LEAPFROG_EUCLIDEAN_ARGS),
+    "mb200_leapfrog_euclidean_generic": (ctypes.c_int, _LEAPFROG_EUCLIDEAN_ARGS),
     "mb200_hamiltonian_euclidean": (ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P]),
     "mb200_euclidean_eval": (ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P, _P, _P, _P]),
     "mb200_constrained_leapfrog_euclidean": (
         ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _I32, _I32, _I32, _P, _MP]
+        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _MP]
         + [_I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P],
     ),
     "mb200_implicit_leapfrog_riemannian": (
         ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _I32, _MP, _I32, _F64, _F64, _I32, _F64]
+        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _MP, _I32, _F64, _F64, _I32, _F64]
         + [_P, _P, _P, _P, _P, _I64, _P],
     ),
     "mb200_implicit_workspace_bytes": (_I64, [_I64, _I32, _MP]),
@@ -88,14 +86,10 @@ SIGNATURES = {
         ctypes.c_int,
         [_I32, _I32, _P, _P, _I64, _I32, _F64, _F64, _I32, _P, _P, _P, _P],
     ),
-    "mb200_composition_euclidean": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _I32, _I32, _P, _I32, _I32, _P, _MP, _P, _P, _P, _P],
-    ),
     "mb200_selftest_eigh": (ctypes.c_int, [_P, _I64, _I32, _I32, _P, _P, _P, _P]),
     "mb200_implicit_midpoint_riemannian": (
         ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _I32, _MP, _I32, _F64, _F64, _I32, _F64]
+        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _MP, _I32, _F64, _F64, _I32, _F64]
         + [_P, _P, _P, _P, _P],
     ),
     "mb200_project_onto_cotangent_space": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P]),
@@ -112,24 +106,10 @@ SIGNATURES = {
     "mb200_nuts_generic_finish": (ctypes.c_int, [_I64, _I32, _I32, _NP, _P, _P, _P]),
     "mb200_nuts_generic_end": (
         ctypes.c_int, [_I64, _I32, _NP, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
-    "mb200_leapfrog_euclidean_per_chain": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _P, _P, _I32, _I32, _P, _I32, _I32, _P, _MP, _P, _P, _P, _P],
-    ),
     "mb200_leapfrog_gaussian_euclidean": (
         ctypes.c_int,
         [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _I32, _P, _I32, _I32, _P, _P, _MP, _P, _P,
          _P, _P],
-    ),
-    "mb200_constrained_leapfrog_euclidean_per_chain": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _P, _P, _I32, _I32, _I32, _P, _MP, _I32, _F64, _F64, _F64,
-         _I32, _I32, _F64, _P, _P, _P, _P, _P],
-    ),
-    "mb200_implicit_riemannian_per_chain": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _P, _P, _I32, _I32, _MP, _I32, _F64, _F64, _I32, _F64, _P,
-         _P, _P, _P, _P],
     ),
     "mb200_nuts_workspace_bytes": (ctypes.c_int64, [_I64, _I32, _I32]),
     "mb200_nuts_euclidean": (

@@ -9,7 +9,8 @@ single ``all_gather`` of the per-rank partial statistics (the only collective of
 window; pass ``group=`` or rely on the default process group).
 
 * ``DualAveragingStepSizeAdapter``   adapters.py:172-391: per-chain dual averaging; the integrator
-  carries a per-chain step-size tensor while it runs (``mb200_leapfrog_euclidean_per_chain``),
+  carries a per-chain step-size tensor while it runs (the ``step_sizes`` array of the integrator
+  entry points),
   ``finalize`` reduces the smoothed log step sizes to the one shared step size of the main stage.
 * ``OnlineVarianceMetricAdapter``    adapters.py:394-518: Welford per chain, Chan et al. merge.
 * ``OnlineCovarianceMetricAdapter``  adapters.py:521-648: Welford per chain, Schubert-Gertz merge.

@@ -26,21 +26,16 @@ inline int check_launch(const char* what) {
   return 0;
 }
 
-// Per-chain overrides travel from the *_per_chain entry points to the kernels through the calling
-// thread only (thread-local, scoped): the plain entry points stay re-entrant and unchanged.
-inline thread_local const double* tl_step_sizes = nullptr;
-inline thread_local const int32_t* tl_n_steps = nullptr;
 inline thread_local int32_t* tl_counters = nullptr;  // mb200_set_call_counters
-struct PerChainScope {
-  PerChainScope(const double* eps, const int32_t* ns) { tl_step_sizes = eps, tl_n_steps = ns; }
-  ~PerChainScope() { tl_step_sizes = nullptr, tl_n_steps = nullptr; }
-};
 
-inline ModelArgs to_args(const mb200_model* m) {
+// Kernel arguments of a model.  step_sizes / n_steps_pc: the optional per-chain device arrays of
+// the implicit and constrained entry points (NULL: every chain uses the scalar argument).
+inline ModelArgs to_args(const mb200_model* m, const double* step_sizes = nullptr,
+                         const int32_t* n_steps_pc = nullptr) {
   ModelArgs a;
   memset(&a, 0, sizeof(a));
-  a.step_sizes = tl_step_sizes;
-  a.n_steps_pc = tl_n_steps;
+  a.step_sizes = step_sizes;
+  a.n_steps_pc = n_steps_pc;
   a.counters = tl_counters;
   a.target_id = m->target_id;
   for (int i = 0; i < MB200_MAX_PARAMS; ++i) a.tp[i] = m->target_params[i];
@@ -84,7 +79,7 @@ struct DeviceScope {
 
 // Workspace: caller-provided when large enough, else a stream-ordered allocation that is freed
 // (stream-ordered) right after the launch -- entry points without a workspace parameter
-// (momentum refresh, velocity, per-chain variants) use the latter.
+// (momentum refresh, velocity, implicit midpoint) use the latter.
 struct DgScratch {
   double* ptr = nullptr;
   bool owned = false;

@@ -48,11 +48,12 @@ extern "C" {
 
 int mb200_constrained_leapfrog_euclidean(
     const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, int32_t n_steps,
-    int32_t n_inner_step, int32_t metric_kind, const double* metric_inv, const mb200_model* model,
-    int32_t projection_solver, double constraint_tol, double position_tol, double divergence_tol,
-    int32_t max_iters, int32_t max_line_search_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* newton_iters, void* stream) {
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream) {
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
@@ -66,7 +67,7 @@ int mb200_constrained_leapfrog_euclidean(
     return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
   if (n_chains == 0) return 0;
   const DeviceScope device_scope(pos_in);
-  const ModelArgs m = to_args(model);
+  const ModelArgs m = to_args(model, step_sizes, n_steps_per_chain);
   cudaStream_t st = (cudaStream_t)stream;
 #define MB200_ARGS                                                                              \
   pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps, n_inner_step,       \
@@ -158,23 +159,6 @@ int mb200_project_onto_cotangent_space(const double* pos, const double* mom_in, 
       return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
   }
 #undef MB200_ARGS
-}
-
-int mb200_constrained_leapfrog_euclidean_per_chain(
-    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, const double* step_sizes,
-    const int32_t* n_steps_per_chain, int32_t max_n_steps, int32_t n_inner_step,
-    int32_t metric_kind, const double* metric_inv, const mb200_model* model,
-    int32_t projection_solver, double constraint_tol, double position_tol, double divergence_tol,
-    int32_t max_iters, int32_t max_line_search_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* newton_iters, void* stream) {
-  if (n_chains > 0 && !step_sizes) return fail(MB200_ERR_INVALID_ARG, "step_sizes is NULL");
-  PerChainScope scope(step_sizes, n_steps_per_chain);
-  return mb200_constrained_leapfrog_euclidean(
-      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, 0.0, max_n_steps, n_inner_step,
-      metric_kind, metric_inv, model, projection_solver, constraint_tol, position_tol,
-      divergence_tol, max_iters, max_line_search_iters, reverse_check_tol, h_out, status, n_done,
-      newton_iters, stream);
 }
 
 }  // extern "C"

@@ -148,22 +148,35 @@ static int dispatch_generic_dim(const double* q_in, const double* p_in, double* 
   return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported by the Euclidean leapfrog", dim);
 }
 
-static FlowSchedule leapfrog_schedule() {
-  FlowSchedule s;
+// Splitting schedule of the C-ABI arguments: n_flows (odd) coefficients alternating a, b, ..., a
+// with a = h1_flow (kick) if initial_h1_flow_step else h2_flow (drift) (integrators.py:268-281);
+// coefficients == NULL is the leapfrog schedule {0.5 kick, 1 drift, 0.5 kick}.
+static int make_schedule(FlowSchedule& s, int n_flows, const double* coefficients,
+                         int initial_h1_flow_step) {
   memset(&s, 0, sizeof(s));
-  s.n = 3;
-  s.drift_mask = 0x2u;
-  s.coef[0] = 0.5, s.coef[1] = 1.0, s.coef[2] = 0.5;
-  return s;
+  if (coefficients == nullptr) {
+    s.n = 3;
+    s.drift_mask = 0x2u;
+    s.coef[0] = 0.5, s.coef[1] = 1.0, s.coef[2] = 0.5;
+    return 0;
+  }
+  if (n_flows < 1 || n_flows > MB200_MAX_FLOWS || (n_flows & 1) == 0)
+    return fail(MB200_ERR_INVALID_ARG, "n_flows must be odd and in [1, %d]", MB200_MAX_FLOWS);
+  s.n = n_flows;
+  for (int i = 0; i < n_flows; ++i) {
+    s.coef[i] = coefficients[i];
+    const bool is_a = (i & 1) == 0;
+    if (initial_h1_flow_step ? !is_a : is_a) s.drift_mask |= 1u << i;
+  }
+  return 0;
 }
 
 static int leapfrog_euclidean_impl(const double* q_in, const double* p_in, double* q_out,
                                    double* p_out, const int32_t* dir, int64_t n, int dim,
-                                   double eps, int n_steps, int metric_kind, const double* minv,
-                                   const mb200_model* model, double* h_out, int32_t* status,
-                                   int32_t* n_done, cudaStream_t st, bool allow_dmma,
-                                   const FlowSchedule* schedule = nullptr) {
-  const FlowSchedule sched = schedule ? *schedule : leapfrog_schedule();
+                                   double eps, int n_steps, const FlowSchedule& sched,
+                                   int metric_kind, const double* minv, const mb200_model* model,
+                                   double* h_out, int32_t* status, int32_t* n_done,
+                                   cudaStream_t st, bool allow_dmma) {
   if (n == 0 && dim >= 1 && n_steps >= 0) return 0;  // empty batch: nothing to do
   if (!q_in || !p_in || !q_out || !p_out || !model)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
@@ -197,6 +210,26 @@ static int leapfrog_euclidean_impl(const double* q_in, const double* p_in, doubl
                   m.target_id);
   }
 #undef MB200_ARGS
+}
+
+// mb200_leapfrog_euclidean (allow_dmma) and mb200_leapfrog_euclidean_generic
+static int leapfrog_euclidean_entry(const double* q_in, const double* p_in, double* q_out,
+                                    double* p_out, const int32_t* dir, int64_t n, int dim,
+                                    double eps, const double* step_sizes, int n_steps,
+                                    const int32_t* n_steps_pc, int n_flows,
+                                    const double* coefficients, int initial_h1_flow_step,
+                                    int metric_kind, const double* minv, const mb200_model* model,
+                                    double* h_out, int32_t* status, int32_t* n_done,
+                                    cudaStream_t st, bool allow_dmma) {
+  FlowSchedule s;
+  if (const int rc = make_schedule(s, n_flows, coefficients, initial_h1_flow_step)) return rc;
+  s.step_sizes = step_sizes;
+  s.n_steps = n_steps_pc;
+  // the tensor-core kernel runs the leapfrog schedule with one trajectory length; with per-chain
+  // step sizes it scales the momentum tile by eps_c
+  allow_dmma = allow_dmma && coefficients == nullptr && n_steps_pc == nullptr;
+  return leapfrog_euclidean_impl(q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, s,
+                                 metric_kind, minv, model, h_out, status, n_done, st, allow_dmma);
 }
 
 template <class Target, int KP>
@@ -237,25 +270,33 @@ extern "C" {
 
 int mb200_leapfrog_euclidean(const double* pos_in, const double* mom_in, double* pos_out,
                              double* mom_out, const int32_t* dir, int64_t n_chains, int32_t dim,
-                             double step_size, int32_t n_steps, int32_t metric_kind,
-                             const double* metric_inv, const mb200_model* model, double* h_out,
-                             int32_t* status, int32_t* n_done, void* stream) {
-  return leapfrog_euclidean_impl(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                                 n_steps, metric_kind, metric_inv, model, h_out, status, n_done,
-                                 (cudaStream_t)stream, true);
+                             double step_size, const double* step_sizes, int32_t n_steps,
+                             const int32_t* n_steps_per_chain, int32_t n_flows,
+                             const double* coefficients, int32_t initial_h1_flow_step,
+                             int32_t metric_kind, const double* metric_inv,
+                             const mb200_model* model, double* h_out, int32_t* status,
+                             int32_t* n_done, void* stream) {
+  return leapfrog_euclidean_entry(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
+                                  step_sizes, n_steps, n_steps_per_chain, n_flows, coefficients,
+                                  initial_h1_flow_step, metric_kind, metric_inv, model, h_out,
+                                  status, n_done, (cudaStream_t)stream, true);
 }
 
 // Same arithmetic through the general-dimension kernel only (used by tests to cross-check the
 // tensor-core kernel; not part of the reference-facing surface).
 int mb200_leapfrog_euclidean_generic(const double* pos_in, const double* mom_in, double* pos_out,
                                      double* mom_out, const int32_t* dir, int64_t n_chains,
-                                     int32_t dim, double step_size, int32_t n_steps,
-                                     int32_t metric_kind, const double* metric_inv,
-                                     const mb200_model* model, double* h_out, int32_t* status,
-                                     int32_t* n_done, void* stream) {
-  return leapfrog_euclidean_impl(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                                 n_steps, metric_kind, metric_inv, model, h_out, status, n_done,
-                                 (cudaStream_t)stream, false);
+                                     int32_t dim, double step_size, const double* step_sizes,
+                                     int32_t n_steps, const int32_t* n_steps_per_chain,
+                                     int32_t n_flows, const double* coefficients,
+                                     int32_t initial_h1_flow_step, int32_t metric_kind,
+                                     const double* metric_inv, const mb200_model* model,
+                                     double* h_out, int32_t* status, int32_t* n_done,
+                                     void* stream) {
+  return leapfrog_euclidean_entry(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
+                                  step_sizes, n_steps, n_steps_per_chain, n_flows, coefficients,
+                                  initial_h1_flow_step, metric_kind, metric_inv, model, h_out,
+                                  status, n_done, (cudaStream_t)stream, false);
 }
 
 int mb200_hamiltonian_euclidean(const double* pos, const double* mom, int64_t n_chains,
@@ -264,9 +305,10 @@ int mb200_hamiltonian_euclidean(const double* pos, const double* mom, int64_t n_
   if (n_chains == 0 && dim >= 1) return 0;
   if (!h_out) return fail(MB200_ERR_INVALID_ARG, "h_out is NULL");
   // zero leapfrog steps: loads the state, evaluates h, writes the (unchanged) state back in place
-  return leapfrog_euclidean_impl(pos, mom, const_cast<double*>(pos), const_cast<double*>(mom),
-                                 nullptr, n_chains, dim, 0.0, 0, metric_kind, metric_inv, model,
-                                 h_out, nullptr, nullptr, (cudaStream_t)stream, false);
+  return mb200_leapfrog_euclidean_generic(pos, mom, const_cast<double*>(pos),
+                                          const_cast<double*>(mom), nullptr, n_chains, dim, 0.0,
+                                          nullptr, 0, nullptr, 0, nullptr, 0, metric_kind,
+                                          metric_inv, model, h_out, nullptr, nullptr, stream);
 }
 
 int mb200_euclidean_eval(const double* pos, const double* mom, int64_t n_chains, int32_t dim,
@@ -294,60 +336,6 @@ int mb200_euclidean_eval(const double* pos, const double* mom, int64_t n_chains,
 #undef MB200_ARGS
 }
 
-int mb200_composition_euclidean(const double* pos_in, const double* mom_in, double* pos_out,
-                                double* mom_out, const int32_t* dir, int64_t n_chains,
-                                int32_t dim, double step_size, int32_t n_steps, int32_t n_flows,
-                                const double* coefficients, int32_t initial_h1_flow_step,
-                                int32_t metric_kind, const double* metric_inv,
-                                const mb200_model* model, double* h_out, int32_t* status,
-                                int32_t* n_done, void* stream) {
-  if (!coefficients || n_flows < 1 || n_flows > MB200_MAX_FLOWS || (n_flows & 1) == 0)
-    return fail(MB200_ERR_INVALID_ARG, "n_flows must be odd and in [1, %d]", MB200_MAX_FLOWS);
-  FlowSchedule s;
-  memset(&s, 0, sizeof(s));
-  s.n = n_flows;
-  for (int i = 0; i < n_flows; ++i) {
-    s.coef[i] = coefficients[i];
-    const bool is_a = (i & 1) == 0;  // flows alternate a, b, a, ... (integrators.py:279-281)
-    const bool drift = initial_h1_flow_step ? !is_a : is_a;
-    if (drift) s.drift_mask |= 1u << i;
-  }
-  return leapfrog_euclidean_impl(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                                 n_steps, metric_kind, metric_inv, model, h_out, status, n_done,
-                                 (cudaStream_t)stream, false, &s);
-}
-
-int mb200_leapfrog_euclidean_per_chain(const double* pos_in, const double* mom_in, double* pos_out,
-                                       double* mom_out, const int32_t* dir, int64_t n_chains,
-                                       int32_t dim, const double* step_sizes,
-                                       const int32_t* n_steps_per_chain, int32_t max_n_steps,
-                                       int32_t n_flows, const double* coefficients,
-                                       int32_t initial_h1_flow_step, int32_t metric_kind,
-                                       const double* metric_inv, const mb200_model* model,
-                                       double* h_out, int32_t* status, int32_t* n_done,
-                                       void* stream) {
-  if (n_chains > 0 && !step_sizes) return fail(MB200_ERR_INVALID_ARG, "step_sizes is NULL");
-  FlowSchedule s = leapfrog_schedule();
-  if (coefficients != nullptr) {
-    if (n_flows < 1 || n_flows > MB200_MAX_FLOWS || (n_flows & 1) == 0)
-      return fail(MB200_ERR_INVALID_ARG, "n_flows must be odd and in [1, %d]", MB200_MAX_FLOWS);
-    memset(&s, 0, sizeof(s));
-    s.n = n_flows;
-    for (int i = 0; i < n_flows; ++i) {
-      s.coef[i] = coefficients[i];
-      const bool is_a = (i & 1) == 0;
-      if (initial_h1_flow_step ? !is_a : is_a) s.drift_mask |= 1u << i;
-    }
-  }
-  s.step_sizes = step_sizes;
-  s.n_steps = n_steps_per_chain;
-  // plain leapfrog with one trajectory length: the DMMA kernel takes the step sizes per chain
-  const bool dmma_ok = coefficients == nullptr && n_steps_per_chain == nullptr;
-  return leapfrog_euclidean_impl(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, 0.0,
-                                 max_n_steps, metric_kind, metric_inv, model, h_out, status,
-                                 n_done, (cudaStream_t)stream, dmma_ok, &s);
-}
-
 int mb200_leapfrog_gaussian_euclidean(const double* pos_in, const double* mom_in, double* pos_out,
                                       double* mom_out, const int32_t* dir, int64_t n_chains,
                                       int32_t dim, double step_size, const double* step_sizes,
@@ -356,18 +344,8 @@ int mb200_leapfrog_gaussian_euclidean(const double* pos_in, const double* mom_in
                                       const double* metric_inv, const double* rotation,
                                       const mb200_model* model, double* h_out, int32_t* status,
                                       int32_t* n_done, void* stream) {
-  FlowSchedule s = leapfrog_schedule();
-  if (coefficients != nullptr) {
-    if (n_flows < 1 || n_flows > MB200_MAX_FLOWS || (n_flows & 1) == 0)
-      return fail(MB200_ERR_INVALID_ARG, "n_flows must be odd and in [1, %d]", MB200_MAX_FLOWS);
-    memset(&s, 0, sizeof(s));
-    s.n = n_flows;
-    for (int i = 0; i < n_flows; ++i) {
-      s.coef[i] = coefficients[i];
-      const bool is_a = (i & 1) == 0;
-      if (initial_h1_flow_step ? !is_a : is_a) s.drift_mask |= 1u << i;
-    }
-  }
+  FlowSchedule s;
+  if (const int rc = make_schedule(s, n_flows, coefficients, initial_h1_flow_step)) return rc;
   if (metric_kind != MB200_METRIC_IDENTITY && !rotation && n_chains > 0)
     return fail(MB200_ERR_INVALID_ARG, "rotation is NULL");
   if (metric_kind == MB200_METRIC_DENSE && step_sizes)
@@ -377,8 +355,8 @@ int mb200_leapfrog_gaussian_euclidean(const double* pos_in, const double* mom_in
   s.rot = rotation;
   s.step_sizes = step_sizes;
   return leapfrog_euclidean_impl(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                                 n_steps, metric_kind, metric_inv, model, h_out, status, n_done,
-                                 (cudaStream_t)stream, false, &s);
+                                 n_steps, s, metric_kind, metric_inv, model, h_out, status, n_done,
+                                 (cudaStream_t)stream, false);
 }
 
 int64_t mb200_host_scratch_bytes(int64_t n_chains, int32_t dim) {
@@ -451,9 +429,9 @@ int mb200_leapfrog_euclidean_host(const double* pos_in, const double* mom_in, do
         if (dir)
           cudaMemcpyAsync(d_dir + lo, b_dir + lo, len * sizeof(int32_t), cudaMemcpyHostToDevice, st);
         int rc = mb200_leapfrog_euclidean(d_qi + off, d_pi + off, d_qo + off, d_po + off,
-                                          dir ? d_dir + lo : nullptr, len, dim, step_size, n_steps,
-                                          metric_kind, metric_inv, model, nullptr, d_status + lo,
-                                          nullptr, st);
+                                          dir ? d_dir + lo : nullptr, len, dim, step_size, nullptr,
+                                          n_steps, nullptr, 0, nullptr, 0, metric_kind, metric_inv,
+                                          model, nullptr, d_status + lo, nullptr, st);
         if (rc != 0) {
           rcs[c] = rc, msgs[c] = g_err;
           return;
@@ -492,8 +470,8 @@ int mb200_leapfrog_euclidean_host(const double* pos_in, const double* mom_in, do
     if (dir) cudaMemcpyAsync(d_dir + lo, dir + lo, len * sizeof(int32_t), cudaMemcpyHostToDevice, st);
     const int rc = mb200_leapfrog_euclidean(d_qi + off, d_pi + off, d_qo + off, d_po + off,
                                             dir ? d_dir + lo : nullptr, len, dim, step_size,
-                                            n_steps, metric_kind, metric_inv, model, nullptr,
-                                            d_status + lo, nullptr, st);
+                                            nullptr, n_steps, nullptr, 0, nullptr, 0, metric_kind,
+                                            metric_inv, model, nullptr, d_status + lo, nullptr, st);
     if (rc != 0) return rc;
     cudaMemcpyAsync(pos_out + off, d_qo + off, bytes, cudaMemcpyDeviceToHost, st);
     cudaMemcpyAsync(mom_out + off, d_po + off, bytes, cudaMemcpyDeviceToHost, st);

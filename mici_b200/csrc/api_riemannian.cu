@@ -194,11 +194,11 @@ extern "C" {
 
 int mb200_implicit_leapfrog_riemannian(
     const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, int32_t n_steps,
-    const mb200_model* model, int32_t fp_solver, double fp_convergence_tol,
-    double fp_divergence_tol, int32_t fp_max_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* fp_iters, void* workspace, int64_t workspace_bytes,
-    void* stream) {
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* workspace, int64_t workspace_bytes, void* stream) {
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
@@ -206,9 +206,10 @@ int mb200_implicit_leapfrog_riemannian(
     return fail(MB200_ERR_INVALID_ARG, "bad sizes");
   if (n_chains == 0) return 0;
   return implicit_dispatch(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                           n_steps, to_args(model), fp_convergence_tol, fp_divergence_tol,
-                           fp_max_iters, reverse_check_tol, h_out, status, n_done, fp_iters,
-                           (cudaStream_t)stream, 0, fp_solver, workspace, workspace_bytes);
+                           n_steps, to_args(model, step_sizes, n_steps_per_chain),
+                           fp_convergence_tol, fp_divergence_tol, fp_max_iters, reverse_check_tol,
+                           h_out, status, n_done, fp_iters, (cudaStream_t)stream, 0, fp_solver,
+                           workspace, workspace_bytes);
 }
 
 // Per-chain buffers live in shared memory except for the global-workspace dense metric policy
@@ -273,17 +274,19 @@ int mb200_selftest_eigh(const double* matrices, int64_t n_matrices, int32_t dim,
 
 int mb200_implicit_midpoint_riemannian(
     const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, int32_t n_steps,
-    const mb200_model* model, int32_t fp_solver, double fp_convergence_tol,
-    double fp_divergence_tol, int32_t fp_max_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* fp_iters, void* stream) {
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* stream) {
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_chains < 0 || dim < 1 || n_steps < 0 || fp_max_iters < 0)
     return fail(MB200_ERR_INVALID_ARG, "bad sizes");
   return implicit_dispatch(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                           n_steps, to_args(model), fp_convergence_tol, fp_divergence_tol,
+                           n_steps, to_args(model, step_sizes, n_steps_per_chain),
+                           fp_convergence_tol, fp_divergence_tol,
                            fp_max_iters, reverse_check_tol, h_out, status, n_done, fp_iters,
                            (cudaStream_t)stream, 1, fp_solver);
 }
@@ -319,27 +322,6 @@ int mb200_sample_momentum_riemannian(const double* pos, const double* normals, d
   }
 #undef MB200_ARGS
   return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
-}
-
-int mb200_implicit_riemannian_per_chain(
-    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
-    const int32_t* dir, int64_t n_chains, int32_t dim, const double* step_sizes,
-    const int32_t* n_steps_per_chain, int32_t max_n_steps, int32_t midpoint,
-    const mb200_model* model, int32_t fp_solver, double fp_convergence_tol,
-    double fp_divergence_tol, int32_t fp_max_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* fp_iters, void* stream) {
-  if (n_chains > 0 && !step_sizes) return fail(MB200_ERR_INVALID_ARG, "step_sizes is NULL");
-  PerChainScope scope(step_sizes, n_steps_per_chain);
-  if (midpoint)
-    return mb200_implicit_midpoint_riemannian(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim,
-                                              0.0, max_n_steps, model, fp_solver,
-                                              fp_convergence_tol, fp_divergence_tol, fp_max_iters,
-                                              reverse_check_tol, h_out, status, n_done, fp_iters,
-                                              stream);
-  return mb200_implicit_leapfrog_riemannian(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim,
-                                            0.0, max_n_steps, model, fp_solver, fp_convergence_tol,
-                                            fp_divergence_tol, fp_max_iters, reverse_check_tol,
-                                            h_out, status, n_done, fp_iters, nullptr, 0, stream);
 }
 
 int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_out,

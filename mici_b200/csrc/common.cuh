@@ -42,7 +42,7 @@ struct ModelArgs {
   double mp[MB200_MAX_PARAMS];
   const double* maux;
   // optional per-chain overrides of the scalar step_size / n_steps arguments of the implicit and
-  // constrained kernels (device arrays [n_chains] or NULL), set by the *_per_chain entry points
+  // constrained kernels (device arrays [n_chains] or NULL), passed in by their entry points
   const double* step_sizes;
   const int32_t* n_steps_pc;
   // per-CTA global scratch of the global-workspace dense metric policy (dense_global.cuh):

@@ -242,43 +242,54 @@ class TractableFlowIntegrator(Integrator):
             raise ValueError(msg)
         super().__init__(system, step_size)
 
-    def _launch_per_chain(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done,
-                          coefficients=None, initial_h1_flow_step=True):
-        """Per-chain step sizes (``self.step_size`` a ``[n_chains]`` tensor: one dual-averaging
-        state per chain during warm-up, adapters.py:262-283, 373) and / or per-chain trajectory
-        lengths (``n_steps`` an integer tensor: transitions.py:355-412)."""
+    def _launch(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done):
+        """Leapfrog (``self.coefficients is None``) or symmetric composition steps on a Euclidean
+        system, with scalar or per-chain step sizes and trajectory lengths."""
+        sysm = self.system
+        if isinstance(sysm, GaussianEuclideanMetricSystem):
+            return _launch_gaussian(sysm, self.step_size, pos, mom, pos_out, mom_out, dirs,
+                                    n_steps, h, status, n_done, self.coefficients,
+                                    self.initial_h1_flow_step)
         n, dim = pos.shape
         dev = pos.device
-        sysm = self.system
+        eps, eps_t, ns, max_n = _step_args(self.step_size, n_steps, n, dev)
+        coefs, n_flows = _coefficients_arg(self.coefficients)
         model = sysm._model(dev)
-        eps = self.step_size
-        if isinstance(eps, torch.Tensor) and eps.ndim == 1:
-            if eps.shape[0] != n:
-                raise ValueError(f"per-chain step_size has {eps.shape[0]} entries for {n} chains")
-            eps = eps.to(device=dev, dtype=torch.float64).contiguous()
-        else:
-            eps = torch.full((n,), float(eps), dtype=torch.float64, device=dev)
-        if isinstance(n_steps, torch.Tensor):
-            if n_steps.shape != (n,):
-                raise ValueError("per-chain n_steps must have one entry per chain")
-            ns = n_steps.to(device=dev, dtype=torch.int32).contiguous()
-            max_n = int(ns.max().item()) if n > 0 else 0
-        else:
-            ns, max_n = None, int(n_steps)
-        if coefficients is None:
-            coefs, n_flows = None, 0
-        else:
-            coefs = ctypes.cast((ctypes.c_double * len(coefficients))(*coefficients),
-                                ctypes.c_void_p)
-            n_flows = len(coefficients)
-        rc = _lib.load().mb200_leapfrog_euclidean_per_chain(
+        rc = _lib.load().mb200_leapfrog_euclidean(
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, _lib.ptr(eps), _lib.ptr(ns), max_n, n_flows, coefs,
-            1 if initial_h1_flow_step else 0, sysm.metric.kind,
+            n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), n_flows, coefs,
+            1 if self.initial_h1_flow_step else 0, sysm.metric.kind,
             _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model), _lib.ptr(h),
             _lib.ptr(status), _lib.ptr(n_done), _lib.current_stream_ptr(dev),
         )
-        _lib.check(rc, "mb200_leapfrog_euclidean_per_chain")
+        _lib.check(rc, "mb200_leapfrog_euclidean")
+
+
+def _step_args(step_size, n_steps, n, dev):
+    """``(eps, eps_t, ns, max_n)`` of an integrator launch: the scalar step size and trajectory
+    length, and the per-chain device arrays, ``None`` where the argument is a scalar.  A per-chain
+    step size is a ``[n_chains]`` tensor (one dual-averaging state per chain during warm-up,
+    adapters.py:262-283, 373), a per-chain length an integer tensor (transitions.py:355-412)."""
+    if isinstance(step_size, torch.Tensor) and step_size.ndim == 1:
+        if step_size.shape[0] != n:
+            raise ValueError(f"per-chain step_size has {step_size.shape[0]} entries for {n} chains")
+        eps, eps_t = 0.0, step_size.to(device=dev, dtype=torch.float64).contiguous()
+    else:
+        eps, eps_t = float(step_size), None
+    if isinstance(n_steps, torch.Tensor):
+        if n_steps.shape != (n,):
+            raise ValueError("per-chain n_steps must have one entry per chain")
+        ns = n_steps.to(device=dev, dtype=torch.int32).contiguous()
+        return eps, eps_t, ns, (int(ns.max().item()) if n > 0 else 0)
+    return eps, eps_t, None, int(n_steps)
+
+
+def _coefficients_arg(coefficients):
+    """``(HOST array pointer, n_flows)`` of a splitting schedule; ``(None, 0)`` for leapfrog."""
+    if coefficients is None:
+        return None, 0
+    coefs = (ctypes.c_double * len(coefficients))(*coefficients)
+    return ctypes.cast(coefs, ctypes.c_void_p), len(coefficients)
 
 
 def _launch_gaussian(system, step_size, pos, mom, pos_out, mom_out, dirs, n_steps, h, status,
@@ -290,17 +301,14 @@ def _launch_gaussian(system, step_size, pos, mom, pos_out, mom_out, dirs, n_step
     if isinstance(n_steps, torch.Tensor):
         raise NotImplementedError("per-chain trajectory lengths: plain Euclidean systems only")
     model = system._model(dev)
-    per_chain = isinstance(step_size, torch.Tensor) and step_size.ndim == 1
-    eps_t = step_size.to(device=dev, dtype=torch.float64).contiguous() if per_chain else None
-    eps = 0.0 if per_chain else float(step_size)
+    eps, eps_t, _, n_steps = _step_args(step_size, n_steps, n, dev)
+    coefs, n_flows = _coefficients_arg(coefficients)
     if coefficients is None:
-        coefs, n_flows, drift = None, 0, [1.0]
+        drift = [1.0]
     else:
-        coefs = ctypes.cast((ctypes.c_double * len(coefficients))(*coefficients), ctypes.c_void_p)
-        n_flows = len(coefficients)
         first_drift = 1 if initial_h1_flow_step else 0
         drift = list(coefficients[first_drift::2])
-    if per_chain and system.metric.kind == 2:
+    if eps_t is not None and system.metric.kind == 2:
         raise NotImplementedError("per-chain step sizes with a dense Gaussian-split metric")
     rot = system.rotation_device(dev, eps, drift)
     rc = _lib.load().mb200_leapfrog_gaussian_euclidean(
@@ -331,39 +339,6 @@ def _gaussian_flow(system, state, dt):
     state.mom = _like_input(state.mom, mom_out[0] if single else mom_out)
 
 
-def _per_chain_args(step_size, n_steps, n, dev):
-    """``(step_sizes tensor, n_steps tensor or None, max_n_steps)`` for the *_per_chain entries."""
-    if isinstance(step_size, torch.Tensor) and step_size.ndim == 1:
-        if step_size.shape[0] != n:
-            raise ValueError(f"per-chain step_size has {step_size.shape[0]} entries for {n} chains")
-        eps = step_size.to(device=dev, dtype=torch.float64).contiguous()
-    else:
-        eps = torch.full((n,), float(step_size), dtype=torch.float64, device=dev)
-    if isinstance(n_steps, torch.Tensor):
-        if n_steps.shape != (n,):
-            raise ValueError("per-chain n_steps must have one entry per chain")
-        ns = n_steps.to(device=dev, dtype=torch.int32).contiguous()
-        return eps, ns, (int(ns.max().item()) if n > 0 else 0)
-    return eps, None, int(n_steps)
-
-
-def _launch_implicit_per_chain(integrator, midpoint, kw, model, pos, mom, pos_out, mom_out, dirs,
-                               n_steps, h, status, n_done, iters):
-    n, dim = pos.shape
-    dev = pos.device
-    eps, ns, max_n = _per_chain_args(integrator.step_size, n_steps, n, dev)
-    rc = _lib.load().mb200_implicit_riemannian_per_chain(
-        _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs), n, dim,
-        _lib.ptr(eps), _lib.ptr(ns), max_n, midpoint, ctypes.byref(model),
-        integrator.fixed_point_solver.kind, float(kw["convergence_tol"]),
-        float(kw["divergence_tol"]), int(kw["max_iters"]), float(integrator.reverse_check_tol),
-        _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters),
-        _lib.current_stream_ptr(dev),
-    )
-    _lib.check(rc, "mb200_implicit_riemannian_per_chain")
-    return iters
-
-
 def _is_per_chain(step_size, n_steps):
     return (isinstance(step_size, torch.Tensor) and step_size.ndim == 1) or isinstance(
         n_steps, torch.Tensor)
@@ -372,6 +347,10 @@ def _is_per_chain(step_size, n_steps):
 class LeapfrogIntegrator(TractableFlowIntegrator):
     """Explicit leapfrog Psi(t) = Phi_1(t/2) o Phi_2(t) o Phi_1(t/2) (integrators.py:134-173)
     for ``EuclideanMetricSystem`` s, target gradient and metric product fused in one kernel."""
+
+    # splitting schedule of TractableFlowIntegrator._launch: None is leapfrog {0.5, 1, 0.5}
+    coefficients = None
+    initial_h1_flow_step = True
 
     def __init__(self, system, step_size=None):
         super().__init__(system, step_size)
@@ -424,25 +403,6 @@ class LeapfrogIntegrator(TractableFlowIntegrator):
         _lib.check(rc, "mb200_leapfrog_euclidean_host")
         return True
 
-    def _launch(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done):
-        if isinstance(self.system, GaussianEuclideanMetricSystem):
-            return _launch_gaussian(self.system, self.step_size, pos, mom, pos_out, mom_out, dirs,
-                                    n_steps, h, status, n_done)
-        if _is_per_chain(self.step_size, n_steps):
-            return self._launch_per_chain(pos, mom, pos_out, mom_out, dirs, n_steps, h, status,
-                                          n_done)
-        n, dim = pos.shape
-        dev = pos.device
-        sysm = self.system
-        model = sysm._model(dev)
-        rc = _lib.load().mb200_leapfrog_euclidean(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, float(self.step_size), n_steps, sysm.metric.kind,
-            _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model), _lib.ptr(h),
-            _lib.ptr(status), _lib.ptr(n_done), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_leapfrog_euclidean")
-
 
 class SymmetricCompositionIntegrator(TractableFlowIntegrator):
     """Symmetric composition (splitting) integrator for ``EuclideanMetricSystem`` s
@@ -463,28 +423,6 @@ class SymmetricCompositionIntegrator(TractableFlowIntegrator):
         coefficients.append(0.5 - sum(free_coefficients[(n_free_coefficients) % 2 :: 2]))
         coefficients.append(1 - 2 * sum(free_coefficients[(n_free_coefficients + 1) % 2 :: 2]))
         self.coefficients = coefficients + coefficients[-2::-1]
-
-    def _launch(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done):
-        if isinstance(self.system, GaussianEuclideanMetricSystem):
-            return _launch_gaussian(self.system, self.step_size, pos, mom, pos_out, mom_out, dirs,
-                                    n_steps, h, status, n_done, self.coefficients,
-                                    self.initial_h1_flow_step)
-        if _is_per_chain(self.step_size, n_steps):
-            return self._launch_per_chain(pos, mom, pos_out, mom_out, dirs, n_steps, h, status,
-                                          n_done, self.coefficients, self.initial_h1_flow_step)
-        n, dim = pos.shape
-        dev = pos.device
-        sysm = self.system
-        model = sysm._model(dev)
-        coefs = (ctypes.c_double * len(self.coefficients))(*self.coefficients)
-        rc = _lib.load().mb200_composition_euclidean(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, float(self.step_size), n_steps, len(self.coefficients),
-            ctypes.cast(coefs, ctypes.c_void_p), 1 if self.initial_h1_flow_step else 0,
-            sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model),
-            _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_composition_euclidean")
 
 
 class BCSSTwoStageIntegrator(SymmetricCompositionIntegrator):
@@ -514,93 +452,71 @@ class BCSSFourStageIntegrator(SymmetricCompositionIntegrator):
         super().__init__(system, (a_0, b_1, a_1), step_size=step_size, initial_h1_flow_step=True)
 
 
-class ImplicitLeapfrogIntegrator(Integrator):
+class _ImplicitIntegrator(Integrator):
+    """Implicit integrators on ``RiemannianMetricSystem`` s: the fixed-point solves and the
+    reversibility check run inside the kernel."""
+
+    _ENTRY = None  # C entry point
+    _WORKSPACE = False  # whether the entry point takes the system's workspace
+
+    def __init__(self, system, step_size=None, reverse_check_tol=2e-8,
+                 reverse_check_norm=maximum_norm, fixed_point_solver=solve_fixed_point_direct,
+                 fixed_point_solver_kwargs=None):
+        super().__init__(system, step_size)
+        if not isinstance(system, RiemannianMetricSystem):
+            raise TypeError(f"{type(self).__name__} needs a RiemannianMetricSystem.")
+        if reverse_check_norm is not maximum_norm:
+            raise ValueError("Only `maximum_norm` is available for the reversibility check.")
+        if fixed_point_solver not in _FUSED_FIXED_POINT_SOLVERS:
+            raise ValueError("Only `solve_fixed_point_direct` and `solve_fixed_point_steffensen` "
+                             "are fused into the kernels.")
+        self.reverse_check_tol = reverse_check_tol
+        self.reverse_check_norm = reverse_check_norm
+        self.fixed_point_solver = fixed_point_solver
+        self.fixed_point_solver_kwargs = dict(fixed_point_solver_kwargs or {})
+
+    def _launch(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done):
+        n, dim = pos.shape
+        dev = pos.device
+        sysm = self.system
+        kw = self.fixed_point_solver.resolve_kwargs(self.fixed_point_solver_kwargs)
+        model = sysm._model(dev)
+        eps, eps_t, ns, max_n = _step_args(self.step_size, n_steps, n, dev)
+        iters = torch.zeros((n, 4), dtype=torch.int32, device=dev)
+        if self._WORKSPACE:
+            ws = sysm._workspace(n, dim, dev)
+            ws_args = (_lib.ptr(ws), ws.numel())
+        else:
+            ws_args = ()
+        rc = getattr(_lib.load(), self._ENTRY)(
+            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
+            n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), ctypes.byref(model),
+            self.fixed_point_solver.kind, float(kw["convergence_tol"]),
+            float(kw["divergence_tol"]), int(kw["max_iters"]),
+            float(self.reverse_check_tol), _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done),
+            _lib.ptr(iters), *ws_args, _lib.current_stream_ptr(dev),
+        )
+        _lib.check(rc, self._ENTRY)
+        return iters
+
+
+class ImplicitLeapfrogIntegrator(_ImplicitIntegrator):
     """Implicit generalised leapfrog for non-separable Hamiltonians (integrators.py:381-544),
     for ``RiemannianMetricSystem`` s.  Fixed-point solves and reversibility checks run inside
     the kernel.  NB: as in the reference at this commit every sub-map receives the full
     ``dir * step_size`` (integrators.py:538-544; SURVEY.md H3)."""
 
-    def __init__(self, system, step_size=None, reverse_check_tol=2e-8,
-                 reverse_check_norm=maximum_norm, fixed_point_solver=solve_fixed_point_direct,
-                 fixed_point_solver_kwargs=None):
-        super().__init__(system, step_size)
-        if not isinstance(system, RiemannianMetricSystem):
-            raise TypeError("ImplicitLeapfrogIntegrator needs a RiemannianMetricSystem.")
-        if reverse_check_norm is not maximum_norm:
-            raise ValueError("Only `maximum_norm` is available for the reversibility check.")
-        if fixed_point_solver not in _FUSED_FIXED_POINT_SOLVERS:
-            raise ValueError("Only `solve_fixed_point_direct` and `solve_fixed_point_steffensen` "
-                             "are fused into the kernels.")
-        self.reverse_check_tol = reverse_check_tol
-        self.reverse_check_norm = reverse_check_norm
-        self.fixed_point_solver = fixed_point_solver
-        self.fixed_point_solver_kwargs = dict(fixed_point_solver_kwargs or {})
-
-    def _launch(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done):
-        n, dim = pos.shape
-        dev = pos.device
-        sysm = self.system
-        kw = self.fixed_point_solver.resolve_kwargs(self.fixed_point_solver_kwargs)
-        model = sysm._model(dev)
-        iters = torch.zeros((n, 4), dtype=torch.int32, device=dev)
-        if _is_per_chain(self.step_size, n_steps):
-            return _launch_implicit_per_chain(self, 0, kw, model, pos, mom, pos_out, mom_out, dirs,
-                                              n_steps, h, status, n_done, iters)
-        ws = sysm._workspace(n, dim, dev)
-        rc = _lib.load().mb200_implicit_leapfrog_riemannian(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, float(self.step_size), n_steps, ctypes.byref(model),
-            self.fixed_point_solver.kind, float(kw["convergence_tol"]),
-            float(kw["divergence_tol"]), int(kw["max_iters"]),
-            float(self.reverse_check_tol), _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done),
-            _lib.ptr(iters), _lib.ptr(ws), ws.numel(), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_implicit_leapfrog_riemannian")
-        return iters
+    _ENTRY = "mb200_implicit_leapfrog_riemannian"
+    _WORKSPACE = True
 
 
-class ImplicitMidpointIntegrator(Integrator):
+class ImplicitMidpointIntegrator(_ImplicitIntegrator):
     """Implicit midpoint integrator for general Hamiltonians (integrators.py:547-681) --
     "next" row N4 -- for ``RiemannianMetricSystem`` s: a fixed-point solve in ``(q, p)`` for the
     forward half-step, an explicit Euler half-step and a reversibility check, all inside the
     kernel.  Same constructor as the reference."""
 
-    def __init__(self, system, step_size=None, reverse_check_tol=2e-8,
-                 reverse_check_norm=maximum_norm, fixed_point_solver=solve_fixed_point_direct,
-                 fixed_point_solver_kwargs=None):
-        super().__init__(system, step_size)
-        if not isinstance(system, RiemannianMetricSystem):
-            raise TypeError("ImplicitMidpointIntegrator needs a RiemannianMetricSystem.")
-        if reverse_check_norm is not maximum_norm:
-            raise ValueError("Only `maximum_norm` is available for the reversibility check.")
-        if fixed_point_solver not in _FUSED_FIXED_POINT_SOLVERS:
-            raise ValueError("Only `solve_fixed_point_direct` and `solve_fixed_point_steffensen` "
-                             "are fused into the kernels.")
-        self.reverse_check_tol = reverse_check_tol
-        self.reverse_check_norm = reverse_check_norm
-        self.fixed_point_solver = fixed_point_solver
-        self.fixed_point_solver_kwargs = dict(fixed_point_solver_kwargs or {})
-
-    def _launch(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done):
-        n, dim = pos.shape
-        dev = pos.device
-        sysm = self.system
-        kw = self.fixed_point_solver.resolve_kwargs(self.fixed_point_solver_kwargs)
-        model = sysm._model(dev)
-        iters = torch.zeros((n, 4), dtype=torch.int32, device=dev)
-        if _is_per_chain(self.step_size, n_steps):
-            return _launch_implicit_per_chain(self, 1, kw, model, pos, mom, pos_out, mom_out, dirs,
-                                              n_steps, h, status, n_done, iters)
-        rc = _lib.load().mb200_implicit_midpoint_riemannian(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, float(self.step_size), n_steps, ctypes.byref(model),
-            self.fixed_point_solver.kind, float(kw["convergence_tol"]),
-            float(kw["divergence_tol"]), int(kw["max_iters"]),
-            float(self.reverse_check_tol), _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done),
-            _lib.ptr(iters), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_implicit_midpoint_riemannian")
-        return iters
+    _ENTRY = "mb200_implicit_midpoint_riemannian"
 
 
 class ConstrainedLeapfrogIntegrator(TractableFlowIntegrator):
@@ -631,30 +547,16 @@ class ConstrainedLeapfrogIntegrator(TractableFlowIntegrator):
         sysm = self.system
         kw = self.projection_solver.resolve_kwargs(self.projection_solver_kwargs)
         model = sysm._model(dev)
+        eps, eps_t, ns, max_n = _step_args(self.step_size, n_steps, n, dev)
         iters = torch.zeros(n, dtype=torch.int32, device=dev)
-        if _is_per_chain(self.step_size, n_steps):
-            eps, ns, max_n = _per_chain_args(self.step_size, n_steps, n, dev)
-            rc = _lib.load().mb200_constrained_leapfrog_euclidean_per_chain(
-                _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out),
-                _lib.ptr(dirs), n, dim, _lib.ptr(eps), _lib.ptr(ns), max_n,
-                int(self.n_inner_step), sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(dev)),
-                ctypes.byref(model), self.projection_solver.kind, float(kw["constraint_tol"]),
-                float(kw["position_tol"]), float(kw["divergence_tol"]), int(kw["max_iters"]),
-                int(kw.get("max_line_search_iters", 10)), float(self.reverse_check_tol),
-                _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters),
-                _lib.current_stream_ptr(dev),
-            )
-            _lib.check(rc, "mb200_constrained_leapfrog_euclidean_per_chain")
-            return iters
         rc = _lib.load().mb200_constrained_leapfrog_euclidean(
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, float(self.step_size), n_steps, int(self.n_inner_step), sysm.metric.kind,
-            _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model),
+            n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), int(self.n_inner_step),
+            sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model),
             self.projection_solver.kind, float(kw["constraint_tol"]), float(kw["position_tol"]),
             float(kw["divergence_tol"]), int(kw["max_iters"]),
             int(kw.get("max_line_search_iters", 10)), float(self.reverse_check_tol), _lib.ptr(h),
-            _lib.ptr(status),
-            _lib.ptr(n_done), _lib.ptr(iters), _lib.current_stream_ptr(dev),
+            _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters), _lib.current_stream_ptr(dev),
         )
         _lib.check(rc, "mb200_constrained_leapfrog_euclidean")
         return iters

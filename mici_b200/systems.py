@@ -451,8 +451,9 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
         model = self._model(dev)
         rc = _lib.load().mb200_constrained_leapfrog_euclidean(
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(scratch_q), _lib.ptr(scratch_p), None, n, dim,
-            0.0, 0, 1, m.kind, _lib.ptr(m.inv_device(dev)), ctypes.byref(model), 0, 1e-9, 1e-8,
-            1e10, 50, 10, 2e-8, _lib.ptr(h), None, None, None, _lib.current_stream_ptr(dev),
+            0.0, None, 0, None, 1, m.kind, _lib.ptr(m.inv_device(dev)), ctypes.byref(model), 0,
+            1e-9, 1e-8, 1e10, 50, 10, 2e-8, _lib.ptr(h), None, None, None,
+            _lib.current_stream_ptr(dev),
         )
         _lib.check(rc, "mb200_constrained_leapfrog_euclidean")
         return _like_input(state.pos, h[0] if single else h)

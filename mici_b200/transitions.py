@@ -177,7 +177,7 @@ class MetropolisStaticIntegrationTransition(MetropolisIntegrationTransition):
 class MetropolisRandomIntegrationTransition(MetropolisIntegrationTransition):
     """Trajectory length drawn per chain and per transition from ``rng.integers(lower, upper)``
     (transitions.py:355-402; NumPy's ``integers`` excludes ``upper``); all chains still advance
-    in one launch (per-chain ``n_steps``, ``mb200_leapfrog_euclidean_per_chain``)."""
+    in one launch (the ``n_steps_per_chain`` array of the integrator entry points)."""
 
     def __init__(self, system, integrator, n_step_range):
         super().__init__(system, integrator)

@@ -56,9 +56,9 @@ def test_header_argument_counts_match_ctypes():
         assert n == len(argtypes), (name, n, len(argtypes))
 
 
-def test_version_and_error_string_without_gpu(handle):
+def test_abi_version_and_error_string_without_gpu(handle):
     handle.mb200_version.restype = ctypes.c_int
-    assert handle.mb200_version() == 100
+    assert handle.mb200_version() == 101
     handle.mb200_last_error.restype = ctypes.c_char_p
     assert isinstance(handle.mb200_last_error(), bytes)
 

@@ -95,7 +95,7 @@ def test_scalar_negative_direction_and_single_chain_state():
     ("C1", {"n_chains": 70, "dim": 64}, "leapfrog"),
     ("C1", {"n_chains": 9, "dim": 11}, "leapfrog"),
 ])
-def test_outputs_may_alias_inputs(cfg, kw, entry):
+def test_leapfrog_outputs_may_alias_inputs(cfg, kw, entry):
     """include/mici_b200.h: `*_out` may alias `*_in` (in-place update)."""
     problem = problems.make_problem(cfg, **kw)
     integ = engine.build_integrator(problem)
@@ -106,7 +106,7 @@ def test_outputs_may_alias_inputs(cfg, kw, entry):
     model = sysm._model(pos.device)
     rc = _lib.load().mb200_leapfrog_euclidean(
         _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos), _lib.ptr(mom), None, pos.shape[0],
-        pos.shape[1], problem.step_size, 3, sysm.metric.kind,
+        pos.shape[1], problem.step_size, None, 3, None, 0, None, 0, sysm.metric.kind,
         _lib.ptr(sysm.metric.inv_device(pos.device)), ctypes.byref(model), None, None, None,
         _lib.current_stream_ptr(pos.device))
     assert rc == 0
@@ -114,7 +114,7 @@ def test_outputs_may_alias_inputs(cfg, kw, entry):
     assert torch.equal(pos, ref.pos) and torch.equal(mom, ref.mom)
 
 
-def test_invalid_arguments_return_errors_not_crashes():
+def test_invalid_leapfrog_arguments_return_errors_not_crashes():
     lib = _lib.load()
     problem = problems.make_problem("C1", n_chains=4, dim=8)
     integ = engine.build_integrator(problem)
@@ -122,7 +122,8 @@ def test_invalid_arguments_return_errors_not_crashes():
     model = integ.system._model(state.pos.device)
     args = lambda **o: [  # noqa: E731
         _lib.ptr(state.pos), _lib.ptr(state.mom), _lib.ptr(state.pos), _lib.ptr(state.mom), None,
-        o.get("n", 4), o.get("dim", 8), 0.1, o.get("n_steps", 1), o.get("kind", 2),
+        o.get("n", 4), o.get("dim", 8), 0.1, None, o.get("n_steps", 1), None, 0, None, 0,
+        o.get("kind", 2),
         o.get("minv", _lib.ptr(integ.system.metric.inv_device(state.pos.device))),
         ctypes.byref(model), None, None, None, _lib.current_stream_ptr(state.pos.device)]
     assert lib.mb200_leapfrog_euclidean(*args(n=-1)) == -1

@@ -85,7 +85,7 @@ def test_step_n_equals_repeated_step(cfg, kwargs):
     assert torch.equal(fused.pos, s.pos) and torch.equal(fused.mom, s.mom)
 
 
-def test_dmma_and_generic_kernels_agree():
+def test_dmma_and_generic_leapfrog_kernels_agree():
     """The tensor-core leapfrog kernel against the general-dimension kernel (same C ABI)."""
     import ctypes
 
@@ -102,7 +102,8 @@ def test_dmma_and_generic_kernels_agree():
     h = torch.empty(n, dtype=torch.float64, device=DEV)
     rc = _lib.load().mb200_leapfrog_euclidean_generic(
         _lib.ptr(state.pos), _lib.ptr(state.mom), _lib.ptr(q), _lib.ptr(p), None, n, dim,
-        problem.step_size, 10, sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(state.pos.device)),
+        problem.step_size, None, 10, None, 0, None, 0, sysm.metric.kind,
+        _lib.ptr(sysm.metric.inv_device(state.pos.device)),
         ctypes.byref(model), _lib.ptr(h), None, None, _lib.current_stream_ptr(state.pos.device))
     assert rc == 0
     torch.cuda.synchronize()
@@ -552,7 +553,7 @@ def _build_adapters(specs):
 @pytest.mark.parametrize("name", ADAPT_NAMES)
 def test_batched_adaptive_sampling_matches_reference_fixture(name):
     """Row N3 on the device: staged warm-up (windowed stager, per-chain dual-averaging step sizes
-    through ``mb200_leapfrog_euclidean_per_chain``, online variance / covariance metric
+    through ``mb200_leapfrog_euclidean``'s ``step_sizes``, online variance / covariance metric
     adaptation, momentum resampling) + main stage, against the reference's own
     ``StaticMetropolisHMC.sample_chains`` -- every chain consuming its own NumPy stream.
     Discrete outcomes (trajectory lengths, accept / reject, directions) must agree exactly."""
@@ -611,8 +612,9 @@ def test_batched_adaptive_sampling_matches_reference_fixture(name):
 
 
 def test_per_chain_step_sizes_and_lengths_match_individual_launches():
-    """``mb200_leapfrog_euclidean_per_chain``: chain c with step size eps_c and n_c steps equals
-    chain c of a plain launch with the scalar (eps_c, n_c) -- bit for bit on the same kernel."""
+    """``mb200_leapfrog_euclidean`` with per-chain step sizes and lengths: chain c with step size
+    eps_c and n_c steps equals chain c of a plain launch with the scalar (eps_c, n_c) -- bit for
+    bit on the same kernel."""
     problem = problems.make_problem("C1", n_chains=37, dim=48)
     integ = engine.build_integrator(problem)
     state = engine.build_state(problem, DEV)
@@ -645,6 +647,22 @@ def test_per_chain_step_sizes_and_lengths_match_individual_launches():
         integ2.step_size = float(eps2[c])
         ref = integ2.step_n(engine.build_state(problem2, DEV, chains=slice(c, c + 1)), 3)
         assert torch.equal(got2.pos[c], ref.pos[0]) and torch.equal(got2.mom[c], ref.mom[0])
+    # one scalar step size with per-chain lengths (no step-size array); a diagonal metric keeps
+    # the single-chain launches on the same general-dimension kernel
+    problem3 = problems.make_problem("C1", n_chains=11, dim=24, metric_kind="diagonal")
+    integ3 = engine.build_integrator(problem3)
+    st3 = engine.build_state(problem3, DEV)
+    ns3 = rng.integers(0, 7, problem3.n_chains).astype(np.int32)
+    dirs3 = torch.as_tensor(rng.choice([-1, 1], problem3.n_chains).astype(np.int32), device=DEV)
+    st3.dir = dirs3
+    got3 = integ3.step_n(st3, torch.as_tensor(ns3, device=DEV), return_h=True)
+    np.testing.assert_array_equal(got3.n_done.cpu().numpy(), ns3)
+    for c in range(problem3.n_chains):
+        one = engine.build_state(problem3, DEV, chains=slice(c, c + 1))
+        one.dir = dirs3[c:c + 1]
+        ref = integ3.step_n(one, int(ns3[c]), return_h=True)
+        assert torch.equal(got3.pos[c], ref.pos[0]) and torch.equal(got3.mom[c], ref.mom[0])
+        assert torch.equal(got3.h[c], ref.h[0])
 
 
 @pytest.mark.parametrize("dim, n_chains", [(48, 37), (128, 70)])
@@ -767,7 +785,7 @@ def test_gaussian_split_h2_flow_and_energy_match_oracle(metric_kind, dim):
     ("C2", {"n_chains": 6, "dim": 8, "integrator": "implicit_midpoint"}),
 ])
 def test_per_chain_launch_of_implicit_and_constrained_integrators(cfg, kwargs):
-    """The *_per_chain entry points: chain c with (eps_c, n_c) equals chain c of a scalar
+    """Per-chain step sizes and lengths: chain c with (eps_c, n_c) equals chain c of a scalar
     launch with that step size and length -- bit for bit, status and iteration counts included
     (large step sizes make some chains fail)."""
     problem = problems.make_problem(cfg, **kwargs)
