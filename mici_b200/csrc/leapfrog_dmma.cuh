@@ -62,10 +62,14 @@ __device__ __forceinline__ void named_barrier_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
-// Profiling hook (profiles/tools/k1_bench.cu defines it to record clock64 per warp and phase);
-// expands to nothing in the library build.
+// Profiling hooks (profiles/tools/k1_bench.cu defines them to record clock64 per warp and phase;
+// MB200_K1_TRACE_AFTER(phase, x) records once the register x has been computed); they expand to
+// nothing in the library build.
 #ifndef MB200_K1_TRACE
 #define MB200_K1_TRACE(phase)
+#endif
+#ifndef MB200_K1_TRACE_AFTER
+#define MB200_K1_TRACE_AFTER(phase, x)
 #endif
 #ifndef MB200_K1_MARK
 #define MB200_K1_MARK(id)
@@ -123,8 +127,10 @@ struct DmmaSmem {
 // groups lock-step) and the step time is  drift (DMMA-pipe bound) + update phase (issue /
 // latency bound).  The update phase is therefore kept as short as possible: no bounds logic
 // (phantom coordinates are zero and stay zero under every registry target's kick), one FMA chain
-// for the reduction, the per-chain scalar (funnel: exp(-v)) published by its owner instead of
-// being summed, own momenta pre-loaded before the group barrier, two barriers per step.
+// for the reduction, the chains of all tiles issued before any shuffle, the per-chain scalar
+// (funnel: exp(-v)) evaluated for all the group's chains in one pass of the coordinate-0 warp and
+// published instead of being summed, own momenta pre-loaded before the group barrier, two
+// barriers per step.
 //
 // PC = true: per-chain step sizes (adaptive warm-up, adapters.py:40-235 per chain).  sm.A then holds
 // A unscaled (step_size = 1) and the momentum tile holds  s = eps_c * dir * p:
@@ -193,36 +199,66 @@ __device__ __forceinline__ void leapfrog_dmma_group(
   int s = -1;  // current step (read by the profiling hook only)
 
   // ---- update phase, part 1 (before the group barrier): this warp's share of the per-chain
-  // reduction and, on the owner lanes, the per-chain scalar
-  auto publish_partials = [&]() {
+  // reduction and, on the coordinate-0 warp, the per-chain scalar
+  auto tile_sums = [&]() {
+    if (!Target::TILE_SUM) return;
+    // sum of squares over the slice: two FMA chains per row, the chains of all tiles issued
+    // before the shuffles of any
+    double v[MT];
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
-      if (Target::TILE_SUM) {
-        // sum of squares over the slice: two FMA chains per row
-        double t0 = q[mt][0][0] * q[mt][0][0];
-        if (Target::COORD0) t0 = owner ? 0.0 : t0;
-        t0 = fma(q[mt][0][1], q[mt][0][1], t0);
-        double t1 = 0.0;
+      double t0 = q[mt][0][0] * q[mt][0][0];
+      if (Target::COORD0) t0 = owner ? 0.0 : t0;
+      t0 = fma(q[mt][0][1], q[mt][0][1], t0);
+      if (mt == 0) MB200_K1_TRACE_AFTER(6, t0);
+      double t1 = 0.0;
 #pragma unroll
-        for (int nt = 1; nt < NT; ++nt) {
-          double& t = (nt & 1) ? t1 : t0;
-          t = fma(q[mt][nt][0], q[mt][nt][0], t);
-          t = fma(q[mt][nt][1], q[mt][nt][1], t);
-        }
-        double v = t0 + t1;
-        v += __shfl_xor_sync(FULL_MASK, v, 1);
-        v += __shfl_xor_sync(FULL_MASK, v, 2);
-        if (c == 0) sm.psum[row[mt]][w] = v;
+      for (int nt = 1; nt < NT; ++nt) {
+        double& t = (nt & 1) ? t1 : t0;
+        t = fma(q[mt][nt][0], q[mt][nt][0], t);
+        t = fma(q[mt][nt][1], q[mt][nt][1], t);
       }
-      if (Target::ROW_SCALAR && owner) sm.rscal[row[mt]] = target.row_scalar(q[mt][0][0]);
+      v[mt] = t0 + t1;
+    }
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) v[mt] += __shfl_xor_sync(FULL_MASK, v[mt], 1);
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) v[mt] += __shfl_xor_sync(FULL_MASK, v[mt], 2);
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt)
+      if (c == 0) sm.psum[row[mt]][w] = v[mt];
+  };
+  auto publish_partials = [&]() {
+    if (Target::ROW_SCALAR && w == 0) {  // warp-uniform
+      // one pass for all the group's chains: lane 4r + mt evaluates row 8mt + r, whose
+      // coordinate 0 lane 4r holds in q[mt][0][0]; lanes with c >= MT evaluate a dummy
+      double v0 = (c == 0) ? q[0][0][0] : 0.0;
+#pragma unroll
+      for (int mt = 1; mt < MT; ++mt) {
+        const double vm = __shfl_sync(FULL_MASK, q[mt][0][0], lane & ~3);
+        v0 = (c == mt) ? vm : v0;
+      }
+      // the sums and the scalar are independent: in one basic block the scheduler interleaves them
+      tile_sums();
+      const double rs = target.row_scalar(v0);
+      if (c < MT) sm.rscal[row0 + 8 * c + r] = rs;
+    } else {
+      tile_sums();
     }
   };
 
-  // ---- update phase, part 2: s -= (eps/2) * grad l(q), KICKS times (1 or 2: the two half-steps
-  // either side of a step boundary stay two separately rounded updates, systems.py:152), one FMA
-  // per coordinate and kick; then make the new momenta visible to the group.  The first barrier
-  // also orders "all A-fragment reads of sm.P done" before the in-place update.
-  auto kick_and_publish = [&](auto kicks_tag) {
+  // ---- the update phase: part 1, the group barrier, then part 2: s -= (eps/2) * grad l(q),
+  // KICKS times (1 or 2: the two half-steps either side of a step boundary stay two separately
+  // rounded updates, systems.py:152), one FMA per coordinate and kick; then make the new momenta
+  // visible to the group.  The first barrier also orders "all A-fragment reads of sm.P done"
+  // before the in-place update.
+  //
+  // The phase moves every momentum through shared memory twice (load own slots, store them
+  // back): 2 x 64 KB per CTA and step at 64 chains x 128, 1024 cycles at 128 B/clk -- more than
+  // its FP64 work.  So the own-slot loads are issued before part 1, where they overlap the DMMA
+  // drain and the partial sums, and the per-chain scalars of all tiles are loaded before the
+  // first tile's stores, which they would otherwise queue behind.
+  auto update_phase = [&](auto kicks_tag) {
     constexpr int KICKS = decltype(kicks_tag)::value;
     double2 pv[MT][NT];
     if (KICKS > 0) {
@@ -231,19 +267,22 @@ __device__ __forceinline__ void leapfrog_dmma_group(
 #pragma unroll
         for (int nt = 0; nt < NT; ++nt) pv[mt][nt] = pslot(mt, nt);  // own slots: no hazard
     }
+    publish_partials();
     MB200_K1_TRACE(2);
     named_barrier_sync(bar_id, 128);
     MB200_K1_TRACE(3);
     if (KICKS == 0) return;
+    double rs[MT];
+#pragma unroll
+    for (int mt = 0; mt < MT; ++mt) rs[mt] = Target::ROW_SCALAR ? sm.rscal[row[mt]] : 1.0;
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
-      const double rs = Target::ROW_SCALAR ? sm.rscal[row[mt]] : 1.0;
       const double mhm = PC ? mhr[PC ? mt : 0] : mh;
-      const double coef = target.kick_coef(mhm, rs);
+      const double coef = target.kick_coef(mhm, rs[mt]);
       double c00 = coef, a00 = q[mt][0][0];
       if (Target::COORD0 && w == 0) {  // warp-uniform; only the owner lanes differ
         const double4 ps = *reinterpret_cast<const double4*>(&sm.psum[row[mt]][0]);
-        const double g0 = target.grad0(q[mt][0][0], ((ps.x + ps.y) + ps.z) + ps.w, rs);
+        const double g0 = target.grad0(q[mt][0][0], ((ps.x + ps.y) + ps.z) + ps.w, rs[mt]);
         c00 = owner ? mhm : coef;
         a00 = owner ? g0 : a00;
       }
@@ -338,21 +377,18 @@ __device__ __forceinline__ void leapfrog_dmma_group(
   };
 
   MB200_K1_MARK(4);
-  publish_partials();
-  if (n_steps > 0) kick_and_publish(K1{});
-  else kick_and_publish(K0{});
+  if (n_steps > 0) update_phase(K1{});
+  else update_phase(K0{});
   MB200_K1_MARK(5);
   for (s = 0; s < n_steps - 1; ++s) {
     MB200_K1_TRACE(0);
     drift(q);  // h2_flow (systems.py:363): q += dir*eps * (A p)
     MB200_K1_TRACE(1);
-    publish_partials();
-    kick_and_publish(K2{});  // closes step s and (cached gradient) opens step s+1
+    update_phase(K2{});  // closes step s and (cached gradient) opens step s+1
   }
   if (n_steps > 0) {
     drift(q);
-    publish_partials();
-    kick_and_publish(K1{});
+    update_phase(K1{});
   }
 
   MB200_K1_MARK(6);

@@ -15,14 +15,12 @@
 
 namespace mb200 {
 
-// exp(x) with a short dependent chain for the tensor-core kernel, where one lane's exp(-v) sits on
-// the critical path of a 4-warp group's update phase (removing it entirely is worth 1.5 % of the
-// C1 launch; profiles/r02_notes.md): x = k ln2 + r, |r| <= ln2/2, e^r by its degree-13 Taylor
-// polynomial in Estrin form (truncation 4e-18 relative; depth 4 after r instead of libm's 11-deep
-// Horner chain), scaled by 2^k through the exponent bits.  Agrees with libm's exp to ~2 ulp;
-// arguments outside [-700, 700] (or non-finite) take libm's exp.
-__device__ __forceinline__ double exp_short_chain(double x) {
-  if (!(fabs(x) < 700.0)) return exp(x);
+// exp(x) with a short dependent chain for the tensor-core kernel, where the exp(-v) of a group's
+// chains sits on the critical path of the group's update phase: x = k ln2 + r, |r| <= ln2/2, e^r
+// by its degree-13 Taylor polynomial in Estrin form (truncation 4e-18 relative; depth 4 after r
+// instead of libm's 11-deep Horner chain), scaled by 2^k through the exponent bits.  Agrees with libm's exp to ~2 ulp for
+// |x| < 700; exp_short_chain sends the other arguments to libm.
+__device__ __forceinline__ double exp_short_chain_poly(double x) {
   const double t = fma(x, 1.4426950408889634, 6755399441055744.0);  // 2^52 + 2^51: rint in low bits
   const double k = t - 6755399441055744.0;
   double r = fma(k, -6.93147180369123816490e-01, x);   // ln2 high part
@@ -40,6 +38,16 @@ __device__ __forceinline__ double exp_short_chain(double x) {
   const double e = fma(s1, r8, s0);
   const long long bits = __double_as_longlong(e) + ((long long)k << 52);
   return __longlong_as_double(bits);
+}
+
+// Arguments outside [-700, 700] (or non-finite) take libm's exp.  Called by all 32 lanes of a warp
+// at once: the polynomial runs branch-free on every lane, and libm's exp only in a warp-uniform
+// branch, taken when some lane's argument is out of range.
+__device__ __forceinline__ double exp_short_chain(double x) {
+  const bool in_range = fabs(x) < 700.0;
+  const double e = exp_short_chain_poly(in_range ? x : 0.0);
+  if (__any_sync(FULL_MASK, !in_range)) return in_range ? e : exp(x);
+  return e;
 }
 
 struct StdGaussianTarget {
@@ -68,7 +76,8 @@ struct StdGaussianTarget {
 //   LINEAR      grad_i = rs * q_i for every coordinate (but possibly coordinate 0): the kick is
 //               one FMA per coordinate with the per-chain coefficient kick_coef(mh, rs);
 //               otherwise kick_pair_nl(mh, x, y, p0, p1) applies the pair's kick itself
-//   ROW_SCALAR  rs = row_scalar(q[0]) is evaluated once per chain by the owner of coordinate 0
+//   ROW_SCALAR  rs = row_scalar(q[0]) is evaluated once per chain by the warp that holds
+//               coordinate 0, all 32 lanes at once (one chain per lane)
 //   TILE_SUM    S = sum over coordinates of q_i^2 (coordinate 0 excluded when COORD0) is
 //               reduced per chain
 //   COORD0      coordinate 0's gradient is grad0(q[0], S, rs) instead of the generic form

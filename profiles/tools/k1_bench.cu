@@ -11,12 +11,22 @@
 #include <cuda_runtime.h>
 
 #ifdef K1_TRACE
-constexpr int TR_STEPS = 8, TR_PHASES = 6, TR_WARPS = 32;
+#include <algorithm>
+// phases: 0 drift start, 1 drift issued, 6 first accumulator value read (the DMMAs have drained),
+// 2 partials written, 3 reduce barrier passed, 4 kick done, 5 publish barrier passed
+constexpr int TR_STEPS = 8, TR_PHASES = 7, TR_WARPS = 32;
 __device__ long long g_trace[TR_WARPS][TR_STEPS][TR_PHASES];
 #define MB200_K1_TRACE(phase)                                                          \
   do {                                                                                 \
     if (blockIdx.x == 0 && (threadIdx.x & 31) == 0 && s >= 20 && s < 20 + TR_STEPS)    \
       g_trace[threadIdx.x >> 5][s - 20][phase] = clock64();                            \
+  } while (0)
+// the empty asm makes x an operand that must exist before the clock is read, so the timestamp
+// follows the instruction that computes x
+#define MB200_K1_TRACE_AFTER(phase, x)                                                 \
+  do {                                                                                 \
+    asm volatile("" ::"d"(x));                                                         \
+    MB200_K1_TRACE(phase);                                                             \
   } while (0)
 __device__ long long g_mark[2][8];
 __device__ unsigned long long g_gt[2][8];
@@ -116,14 +126,86 @@ int main(int argc, char** argv) {
     for (int w = 0; w < DMMA_THREADS / 32; ++w)
       for (int s = 0; s < TR_STEPS; ++s)
         if (tr[w][s][0] < t0 && tr[w][s][0] > 0) t0 = tr[w][s][0];
-    printf("trace (CTA 0, cycles relative to first event; phases: 0 drift start, 1 drift end, "
-           "2 partials written, 3 reduce barrier passed, 4 kick done, 5 publish barrier passed)\n");
+    printf("trace (CTA 0, cycles relative to first event; phases: 0 drift start, 1 drift issued, "
+           "2 partials written, 3 reduce barrier passed, 4 kick done, 5 publish barrier passed, "
+           "6 first accumulator value read)\n");
     for (int w = 0; w < DMMA_THREADS / 32; ++w)
       for (int s = 0; s < TR_STEPS; ++s) {
         printf("w%02d sp%d g%d s%d:", w, w & 3, w >> 2, s);
         for (int ph = 0; ph < TR_PHASES; ++ph) printf(" %7lld", tr[w][s][ph] - t0);
         printf("\n");
       }
+    // median cycles of each sub-phase, by group and by the warp that holds coordinate 0 (the
+    // kernel's w == 0) versus the other three
+    auto median = [](std::vector<long long> v) {
+      if (v.empty()) return 0.0;
+      std::sort(v.begin(), v.end());
+      const size_t n = v.size();
+      return n & 1 ? (double)v[n / 2] : 0.5 * (v[n / 2 - 1] + v[n / 2]);
+    };
+    // {from, to} phase pairs; step = drift start to the next step's drift start
+    const int sub[][2] = {{0, 1}, {1, 6}, {6, 2}, {2, 3}, {3, 4}, {4, 5}, {6, 5}, {0, 6}};
+    const char* names[] = {"drift issue", "DMMA drain", "partials", "wait bar1",
+                           "kick", "wait bar2", "update", "drift+drain"};
+    const int n_sub = 8;
+    const int groups = DMMA_THREADS / 128;
+    printf("update sub-phases (median cycles over steps 20-%d):\n%-14s", 20 + TR_STEPS - 2, "");
+    for (int i = 0; i < n_sub; ++i) printf(" %11s", names[i]);
+    printf(" %11s\n", "step");
+    for (int g = -1; g < groups; ++g)
+      for (int kind = 0; kind < 3; ++kind) {
+        if ((g < 0) != (kind == 2)) continue;  // per group: w0 / others; overall: all warps
+        std::vector<long long> d[n_sub + 1];
+        for (int wp = 0; wp < DMMA_THREADS / 32; ++wp) {
+          const int grp = wp >> 2, w = ((wp & 3) + grp) & 3;  // the kernel's quarter rotation
+          if (g >= 0 && (grp != g || (w == 0) != (kind == 0))) continue;
+          for (int s = 0; s + 1 < TR_STEPS; ++s) {
+            for (int i = 0; i < n_sub; ++i)
+              d[i].push_back(tr[wp][s][sub[i][1]] - tr[wp][s][sub[i][0]]);
+            d[n_sub].push_back(tr[wp][s + 1][0] - tr[wp][s][0]);
+          }
+        }
+        char label[32];
+        if (g < 0) snprintf(label, sizeof(label), "all warps");
+        else snprintf(label, sizeof(label), "g%d %s", g, kind == 0 ? "w0" : "others");
+        printf("%-14s", label);
+        for (int i = 0; i <= n_sub; ++i) printf(" %11.0f", median(d[i]));
+        printf("\n");
+      }
+    // how far apart the groups are: the spread (latest - earliest) over the groups of the group's
+    // drift start (earliest warp), its last arrival at each barrier and its release.  A group may
+    // run a whole step ahead of the others, so each group's event is the one nearest in time to
+    // group 0's, not the one with the same step index.
+    const int ev[][2] = {{0, 0}, {2, 1}, {3, 0}, {4, 1}, {5, 0}};  // {phase, 1: latest warp}
+    const char* ev_names[] = {"drift start", "bar1 arrival", "bar1 release", "bar2 arrival",
+                              "bar2 release"};
+    auto group_event = [&](int g, int s, int e) {
+      long long t = ev[e][1] ? -(1LL << 62) : (1LL << 62);
+      for (int k = 0; k < 4; ++k) {
+        const long long x = tr[4 * g + k][s][ev[e][0]];
+        t = ev[e][1] ? std::max(t, x) : std::min(t, x);
+      }
+      return t;
+    };
+    printf("group skew (median over steps of max - min over the groups, cycles):");
+    for (int e = 0; e < 5; ++e) {
+      std::vector<long long> spread;
+      for (int s = 1; s + 1 < TR_STEPS; ++s) {
+        const long long ref = group_event(0, s, e);
+        long long lo = ref, hi = ref;
+        for (int g = 1; g < groups; ++g) {
+          long long best = group_event(g, 0, e);
+          for (int s2 = 1; s2 < TR_STEPS; ++s2) {
+            const long long t = group_event(g, s2, e);
+            if (std::llabs(t - ref) < std::llabs(best - ref)) best = t;
+          }
+          lo = std::min(lo, best), hi = std::max(hi, best);
+        }
+        spread.push_back(hi - lo);
+      }
+      printf("  %s %.0f", ev_names[e], median(spread));
+    }
+    printf("\n");
   }
 #endif
   return 0;
