@@ -276,6 +276,13 @@ int mb200_selftest_dense_factor(const double* matrices, const double* rhs, int64
                                 double* logdet_out, int32_t* status, void* stream);
 
 /*
+ * Diagnostic: y[i] = exp(x[i]) as the tensor-core leapfrog evaluates it (the funnel's exp(-v) in
+ * K1: a short-chain polynomial for |x| < 700, libm's exp otherwise), one element per thread in
+ * warps of 32 consecutive elements; x and y are device arrays [n].
+ */
+int mb200_selftest_exp_short_chain(const double* x, double* y, int64_t n, void* stream);
+
+/*
  * "Next" row N4: n_steps implicit-midpoint steps on a Riemannian-metric system.
  * Replaces: ImplicitMidpointIntegrator.step (integrators.py:547-681): a direct fixed-point solve
  * in z = (q, p) for the forward half-step, an explicit Euler half-step, and a reversibility

@@ -96,6 +96,7 @@ SIGNATURES = {
     "mb200_sample_momentum_riemannian": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _MP, _P, _P]),
     "mb200_dh_dmom_riemannian": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _MP, _P, _P]),
     "mb200_selftest_dense_factor": (ctypes.c_int, [_P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
+    "mb200_selftest_exp_short_chain": (ctypes.c_int, [_P, _P, _I64, _P]),
     "mb200_nuts_generic_state_bytes": (ctypes.c_int64, [_I64]),
     "mb200_nuts_generic_begin": (
         ctypes.c_int, [_P, _P, _P, _P, _I64, _I32, _NP, _P, _I64, _P, _I64, _P]),

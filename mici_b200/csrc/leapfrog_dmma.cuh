@@ -30,6 +30,7 @@
 //     synchronise only internally (named barriers), so while one group is in its gradient /
 //     update phase the other three keep the sub-partition's DMMA pipe fed.
 #pragma once
+#include <cfloat>
 #include <type_traits>
 
 #include "targets.cuh"
@@ -412,6 +413,8 @@ __device__ __forceinline__ void leapfrog_dmma_group(
             pv.x = p_in[(size_t)ch * dim + i];
             pv.y = (i + 1 < dim) ? p_in[(size_t)ch * dim + i + 1] : 0.0;
           }
+          // eps_c^2 zero or subnormal: the energy epilogue contracts the stored p itself
+          if (h_out != nullptr && !(sgn * sgn >= DBL_MIN)) pslot(mt, nt) = pv;
         }
         if (vec2) {
           *reinterpret_cast<double2*>(q_out + (size_t)ch * dim + i) =
@@ -433,8 +436,14 @@ __device__ __forceinline__ void leapfrog_dmma_group(
 
   MB200_K1_MARK(7);
   // ---- Hamiltonian of the final state: l(q) + p . (A p) / 2   (systems.py:187-196, 348-350)
-  // sm.psum / sm.rscal hold the reduction of the final positions (last update phase)
+  // sm.psum / sm.rscal hold the reduction of the final positions (last update phase).  Without
+  // per-chain step sizes sm.P holds s = dir p against eps A, and s . (eps A) s / eps = p . A p.
+  // With them A is unscaled and a row of sm.P holds s = eps_c dir p, and s . A s / eps_c^2 = p . A p
+  // -- except where eps_c^2 is zero or subnormal (0/0 for eps_c = 0, few significant bits below
+  // |eps_c| = 2^-511): those rows were overwritten with the stored p above, and their kinetic
+  // term is p . A p directly.  (Rows are independent in the contraction.)
   if (h_out != nullptr) {
+    if (PC) named_barrier_sync(bar_id, 128);  // every warp's rows are in sm.P before drift(u)
     double l[MT], kin[MT], u[MT][NT][2];
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
@@ -452,7 +461,7 @@ __device__ __forceinline__ void leapfrog_dmma_group(
         u[mt][nt][0] = 0.0, u[mt][nt][1] = 0.0;
       }
     }
-    drift(u);  // u = s . (eps A); sm.P holds the final momenta
+    drift(u);  // u = s . (eps A)
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) {
       kin[mt] = 0.0;
@@ -480,9 +489,9 @@ __device__ __forceinline__ void leapfrog_dmma_group(
         const double4 l4 = *reinterpret_cast<const double4*>(&sm.ex[1][row[mt]][0]);
         const double ks = ((k4.x + k4.y) + k4.z) + k4.w;
         const double ls = ((l4.x + l4.y) + l4.z) + l4.w;
-        if (PC) {  // ks = eps_c^2 p.A p  (p.A p itself is unavailable for eps_c = 0: NaN)
+        if (PC) {  // ks = eps_c^2 p.A p, or p.A p where eps_c^2 is zero or subnormal
           const double e = step_sizes[chain0 + row[mt]];
-          h_out[chain0 + row[mt]] = ls + 0.5 * (ks / (e * e));
+          h_out[chain0 + row[mt]] = ls + 0.5 * (e * e >= DBL_MIN ? ks / (e * e) : ks);
         } else {
           h_out[chain0 + row[mt]] = ls + 0.5 * (ks / step_size);
         }
