@@ -77,6 +77,11 @@ extern "C" {
 #define MB200_RMETRIC_SOFTABS 0 /* SoftAbs of target Hessian (matrices.py:1631-1685); params: softabs_coeff */
 #define MB200_RMETRIC_RANK1 1   /* dense M(q) = B + c q q^T;  aux: [B | B^-1] (2*dim*dim), params: c, log|B|, force_woodbury, generic_rank1_vjp */
 #define MB200_RMETRIC_HADAMARD 2 /* dense M(q) = B + c (q q^T) o S (full rank); aux: [B | S] (2*dim*dim), params: c, -, -, generic_rank1_vjp */
+/* O(D) metrics (DiagonalRiemannianMetricSystem / ScalarRiemannianMetricSystem, systems.py:1405-1571);
+ * targets: std-Gaussian, banana, funnel, quadratic (the funnel Fisher metric: funnel only) */
+#define MB200_RMETRIC_DIAG_QUADRATIC 3     /* diagonal d_i = a + b q_i^2;  params: a > 0, b >= 0 */
+#define MB200_RMETRIC_DIAG_FUNNEL_FISHER 4 /* diagonal d = [1/9 + (D-1)/2, e^-v, ..., e^-v], v = q[0]: the funnel's expected Fisher information */
+#define MB200_RMETRIC_SCALAR_QUADRATIC 5   /* scaled identity s I, s = a + b |q|^2;  params: a > 0, b >= 0 */
 
 /* fixed-point solvers fused into the implicit integrators (solvers.py:47-94, 97-154) */
 #define MB200_FP_SOLVER_DIRECT 0

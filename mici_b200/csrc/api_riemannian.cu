@@ -16,8 +16,13 @@ static int launch_implicit(const double* q_in, const double* p_in, double* q_out
   // SoftAbs: a third matrix enables warm-started eigensolves; use it when two CTAs still fit
   if (MetricT<Target>::SOFTABS && rm_smem_doubles(dim, 3) * sizeof(double) <= 113 * 1024) n_mats = 3;
   if (MetricT<Target>::SOFTABS && Target::DENSE_MTP) n_mats = 3;  // the third holds Z = A U
-  size_t smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
+  constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
+  size_t smem = (compact ? rm_compact_doubles(dim, midpoint) : rm_smem_doubles(dim, n_mats)) *
+                sizeof(double);
   bool in_ws = false;
+  if (compact && smem > 227 * 1024)
+    return fail(MB200_ERR_UNSUPPORTED, "dim %d: per-chain vectors (%zu bytes) exceed shared memory",
+                dim, smem);
   if (smem > 227 * 1024) {
     // SoftAbs beyond shared memory: the same kernels with the matrices in a per-CTA global
     // workspace (L2-resident operands: slower, but the reference has no dimension limit)
@@ -45,10 +50,9 @@ static int launch_implicit(const double* q_in, const double* p_in, double* q_out
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
-  kern<<<(unsigned)blocks, RM_THREADS, smem, st>>>(q_in, p_in, q_out, p_out, dir, n, dim, eps,
-                                                   n_steps, margs, fp_tol, fp_div, fp_max, rev_tol,
-                                                   h_out, status, n_done, fp_iters, n_mats,
-                                                   midpoint, fp_solver);
+  kern<<<(unsigned)blocks, MetricT<Target>::THREADS, smem, st>>>(
+      q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, margs, fp_tol, fp_div, fp_max, rev_tol,
+      h_out, status, n_done, fp_iters, n_mats, midpoint, fp_solver);
   return check_launch("implicit_leapfrog_kernel");
 }
 
@@ -63,6 +67,71 @@ static bool wants_global_dense(const ModelArgs& m, int dim) {
   return !fits && m.mp[2] == 0.0 && m.target_id == MB200_TARGET_QUADRATIC &&
          dense_global_supported(dim);
 }
+
+static bool is_compact_rmetric(int id) {
+  return id == MB200_RMETRIC_DIAG_QUADRATIC || id == MB200_RMETRIC_DIAG_FUNNEL_FISHER ||
+         id == MB200_RMETRIC_SCALAR_QUADRATIC;
+}
+
+// Target / metric pairs of the O(D) metrics.  `L` is one of the launch functors below: its
+// `run<Target, MetricT>()` launches the entry point's kernel for that pair.
+template <class L>
+static int compact_dispatch(const ModelArgs& m, int dim, const L& l) {
+  if (m.rmetric_id != MB200_RMETRIC_DIAG_FUNNEL_FISHER && !(m.mp[0] > 0.0 && m.mp[1] >= 0.0))
+    return fail(MB200_ERR_INVALID_ARG, "metric parameters need a > 0 and b >= 0");
+  if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
+    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
+  if (m.target_id == MB200_TARGET_QUADRATIC && !m.taux)
+    return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
+  if (m.rmetric_id == MB200_RMETRIC_DIAG_FUNNEL_FISHER) {
+    if (m.target_id != MB200_TARGET_NEAL_FUNNEL)
+      return fail(MB200_ERR_UNSUPPORTED, "the funnel Fisher metric needs the funnel target (got %d)",
+                  m.target_id);
+    return l.template run<FunnelRTarget, FunnelFisherMetric>();
+  }
+  const bool diag = m.rmetric_id == MB200_RMETRIC_DIAG_QUADRATIC;
+  switch (m.target_id) {
+    case MB200_TARGET_STD_GAUSSIAN:
+      return diag ? l.template run<StdGaussianRTarget, QuadraticDiagonalMetric>()
+                  : l.template run<StdGaussianRTarget, ScalarMetric>();
+    case MB200_TARGET_BANANA:
+      return diag ? l.template run<BananaRTarget, QuadraticDiagonalMetric>()
+                  : l.template run<BananaRTarget, ScalarMetric>();
+    case MB200_TARGET_NEAL_FUNNEL:
+      return diag ? l.template run<FunnelRTarget, QuadraticDiagonalMetric>()
+                  : l.template run<FunnelRTarget, ScalarMetric>();
+    case MB200_TARGET_QUADRATIC:
+      return diag ? l.template run<QuadraticRTarget, QuadraticDiagonalMetric>()
+                  : l.template run<QuadraticRTarget, ScalarMetric>();
+    default:
+      return fail(MB200_ERR_UNSUPPORTED, "target %d not available with diagonal / scalar metrics",
+                  m.target_id);
+  }
+}
+
+struct ImplicitLaunch {
+  const double *q_in, *p_in;
+  double *q_out, *p_out;
+  const int32_t* dir;
+  int64_t n;
+  int dim;
+  double eps;
+  int n_steps;
+  const ModelArgs& m;
+  double fp_tol, fp_div;
+  int fp_max;
+  double rev_tol;
+  double* h_out;
+  int32_t *status, *n_done, *fp_iters;
+  cudaStream_t st;
+  int midpoint, fp_solver;
+  template <class Target, template <class> class MetricT>
+  int run() const {
+    return launch_implicit<Target, MetricT>(q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, m,
+                                            fp_tol, fp_div, fp_max, rev_tol, h_out, status, n_done,
+                                            fp_iters, st, midpoint, fp_solver);
+  }
+};
 
 static int implicit_dispatch(const double* q_in, const double* p_in, double* q_out, double* p_out,
                              const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
@@ -123,6 +192,11 @@ static int implicit_dispatch(const double* q_in, const double* p_in, double* q_o
     }
   }
 #undef MB200_ARGS
+  if (is_compact_rmetric(m.rmetric_id))
+    return compact_dispatch(m, dim, ImplicitLaunch{q_in, p_in, q_out, p_out, dir, n, dim, eps,
+                                                   n_steps, m, fp_tol, fp_div, fp_max, rev_tol,
+                                                   h_out, status, n_done, fp_iters, st, midpoint,
+                                                   fp_solver});
   return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
 }
 
@@ -131,7 +205,8 @@ static int launch_sample_momentum(const double* q, const double* z, double* p_ou
                                   int dim, const ModelArgs& m, int32_t* status, cudaStream_t st) {
   auto kern = riemannian_sample_momentum_kernel<Target, MetricT>;
   int n_mats = MetricT<Target>::N_MATS;
-  size_t smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
+  constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
+  size_t smem = (compact ? rm_compact_doubles(dim, 0) : rm_smem_doubles(dim, n_mats)) * sizeof(double);
   bool in_ws = false;
   if (smem > 227 * 1024) {
     if (!MetricT<Target>::SOFTABS) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
@@ -143,6 +218,11 @@ static int launch_sample_momentum(const double* q, const double* z, double* p_ou
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
   int64_t blocks = (int64_t)num_sms() * 2;
+  if (compact) {  // small CTAs: as many as fit
+    int per_sm = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, MetricT<Target>::THREADS, smem);
+    blocks = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
+  }
   if (blocks > n) blocks = n;
   ModelArgs margs = m;
   const size_t per_cta = 3 * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
@@ -152,7 +232,8 @@ static int launch_sample_momentum(const double* q, const double* z, double* p_ou
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
-  kern<<<(unsigned)blocks, RM_THREADS, smem, st>>>(q, z, p_out, n, dim, margs, status, n_mats);
+  kern<<<(unsigned)blocks, MetricT<Target>::THREADS, smem, st>>>(q, z, p_out, n, dim, margs, status,
+                                                                  n_mats);
   return check_launch("riemannian_sample_momentum_kernel");
 }
 
@@ -161,7 +242,8 @@ static int launch_velocity(const double* q, const double* p, double* vel, int64_
                            const ModelArgs& m, int32_t* status, cudaStream_t st) {
   auto kern = riemannian_velocity_kernel<Target, MetricT>;
   int n_mats = MetricT<Target>::N_MATS;
-  size_t smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
+  constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
+  size_t smem = (compact ? rm_compact_doubles(dim, 0) : rm_smem_doubles(dim, n_mats)) * sizeof(double);
   bool in_ws = false;
   if (smem > 227 * 1024) {
     if (!MetricT<Target>::SOFTABS) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
@@ -173,6 +255,11 @@ static int launch_velocity(const double* q, const double* p, double* vel, int64_
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
   int64_t blocks = (int64_t)num_sms() * 2;
+  if (compact) {  // small CTAs: as many as fit
+    int per_sm = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, MetricT<Target>::THREADS, smem);
+    blocks = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
+  }
   if (blocks > n) blocks = n;
   ModelArgs margs = m;
   const size_t per_cta = 3 * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
@@ -182,9 +269,27 @@ static int launch_velocity(const double* q, const double* p, double* vel, int64_
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
-  kern<<<(unsigned)blocks, RM_THREADS, smem, st>>>(q, p, vel, n, dim, margs, status, n_mats);
+  kern<<<(unsigned)blocks, MetricT<Target>::THREADS, smem, st>>>(q, p, vel, n, dim, margs, status,
+                                                                  n_mats);
   return check_launch("riemannian_velocity_kernel");
 }
+
+// sqrt(M(q)) v (velocity = false) or M(q)^-1 v (velocity = true) for the compact metrics
+struct VectorLaunch {
+  const double *q, *v;
+  double* out;
+  int64_t n;
+  int dim;
+  const ModelArgs& m;
+  int32_t* status;
+  cudaStream_t st;
+  bool velocity;
+  template <class Target, template <class> class MetricT>
+  int run() const {
+    return velocity ? launch_velocity<Target, MetricT>(q, v, out, n, dim, m, status, st)
+                    : launch_sample_momentum<Target, MetricT>(q, v, out, n, dim, m, status, st);
+  }
+};
 
 }  // namespace mb200
 
@@ -321,6 +426,9 @@ int mb200_sample_momentum_riemannian(const double* pos, const double* normals, d
     }
   }
 #undef MB200_ARGS
+  if (is_compact_rmetric(m.rmetric_id))
+    return compact_dispatch(m, dim, VectorLaunch{pos, normals, mom_out, n_chains, dim, m, status,
+                                                 st, false});
   return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
 }
 
@@ -359,6 +467,9 @@ int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_o
     }
   }
 #undef MB200_ARGS
+  if (is_compact_rmetric(m.rmetric_id))
+    return compact_dispatch(m, dim, VectorLaunch{pos, mom, vel_out, n_chains, dim, m, status, st,
+                                                 true});
   return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
 }
 

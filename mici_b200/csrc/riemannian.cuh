@@ -174,6 +174,34 @@ struct StdGaussianRTarget {
   __device__ void mtp_entries(const Blk&, const double*, const double*, double*) const {}
 };
 
+// Neal's funnel, v = q[0], x = q[1:]: l = v^2/18 + (D-1) v/2 + exp(-v) |x|^2/2 (the expressions
+// of the NumPy model, oracle/targets.py NealFunnel).  No Hessian: diagonal / scalar metrics only.
+struct FunnelRTarget {
+  static constexpr bool DENSE_MTP = false;
+  __device__ void attach(double*) const {}
+  static constexpr bool HAS_HESSIAN = false;
+  static constexpr int NEED = 1;
+  int dim;
+  __device__ FunnelRTarget(const ModelArgs&, int d) : dim(d) {}
+  __device__ double xsq(const Blk& k, const double* q) const {
+    double s = 0.0;
+    for (int i = 1 + k.tid; i < dim; i += k.nthr) s = fma(q[i], q[i], s);
+    return block_sum(k, s);
+  }
+  __device__ double nld(const Blk& k, const double* q) const {
+    const double s = xsq(k, q), v = q[0];
+    return (v * v / 18.0 + 0.5 * (dim - 1) * v) + 0.5 * exp(-v) * s;
+  }
+  __device__ void grad(const Blk& k, const double* q, double* g) const {
+    const double s = xsq(k, q), v = q[0], e = exp(-v);
+    for (int i = k.tid; i < dim; i += k.nthr)
+      g[i] = (i == 0) ? (v / 9.0 + 0.5 * (dim - 1)) - 0.5 * e * s : e * q[i];
+  }
+  __device__ void hess(const Blk&, const double*, double*, int) const {}
+  __device__ __forceinline__ int need_col(int, int) const { return -1; }
+  __device__ void mtp_entries(const Blk&, const double*, const double*, double*) const {}
+};
+
 // l(q) = |q|^2/2 + (gamma/4) sum_m (a_m . q)^4, A = directions [D x D] in global memory (shared
 // by all chains, L2-resident).  Dense Hessian I + 3 gamma A^T diag(s^2) A, s = A q; the
 // matrix-Tressian product mtp(V)_k = 6 gamma sum_m s_m (a_m^T V a_m) a_mk needs the whole of V:
@@ -444,6 +472,54 @@ __device__ inline void rm_carve(RmWork& w, double* s, int dim, int n_mats, Blk& 
   blk.red = s;
   w.extra = s + 40;
 }
+
+// Compact vector set of the O(D) metric policies (COMPACT: diagonal and scalar metrics): the
+// integrator's vectors q p qs ps x0 x1 x2 base v1 v2 v3 plus ev (policy scratch), lam (d(q)) and
+// sa (1 / d(q)); the implicit-midpoint vectors z0 z1 z2 zb zp [2 dpad each] only when `midpoint`
+// is set.  No matrices, no eigensolver or Cholesky buffers: at D = 128 a chain needs 14.6 KB
+// (leapfrog), so that many chains share an SM.
+__host__ __device__ inline size_t rm_compact_doubles(int dim, int midpoint) {
+  const int dpad = (dim + 1) & ~1;
+  return (size_t)(midpoint ? 24 : 14) * dpad + 40;
+}
+
+__device__ inline void rm_carve_compact(RmWork& w, double* s, int dim, int midpoint, Blk& blk) {
+  const int dpad = (dim + 1) & ~1;
+  w.dim = dim;
+  w.ld = dim + 1;
+  w.M1 = w.M2 = w.M3 = nullptr;
+  double** cv[] = {&w.q,  &w.p,  &w.qs, &w.ps, &w.x0, &w.x1, &w.x2,
+                   &w.base, &w.v1, &w.v2, &w.v3, &w.ev, &w.lam, &w.sa};
+  for (auto v : cv) {
+    *v = s;
+    s += dpad;
+  }
+  w.gsa = w.Vn = nullptr;
+  w.rc = w.rs = nullptr;
+  w.top = w.bot = nullptr;
+  if (midpoint) {
+    double** zv[] = {&w.z0, &w.z1, &w.z2, &w.zb, &w.zp};
+    for (auto v : zv) {
+      *v = s;
+      s += 2 * dpad;
+    }
+  } else {
+    w.z0 = w.z1 = w.z2 = w.zb = w.zp = nullptr;
+  }
+  blk.red = s;
+  w.extra = s + 40;
+}
+
+// true for metric policies that declare `static constexpr bool COMPACT = true` (carved by
+// rm_carve_compact); the matrix policies declare nothing and keep rm_carve
+template <class M, class = void>
+struct rm_compact_policy {
+  static constexpr bool value = false;
+};
+template <class M>
+struct rm_compact_policy<M, decltype(void(M::COMPACT))> {
+  static constexpr bool value = M::COMPACT;
+};
 
 // ---------------------------------------------------------------------------------------------
 // K3: symmetric eigendecomposition A = U diag(lam) U^T by parallel cyclic Jacobi.
@@ -1262,6 +1338,172 @@ struct Rank1WoodburyMetric {
 };
 
 // ---------------------------------------------------------------------------------------------
+// O(D) metrics: DiagonalRiemannianMetricSystem (PositiveDiagonalMatrix, matrices.py:709-792) and
+// ScalarRiemannianMetricSystem (PositiveScaledIdentityMatrix, matrices.py:595-706).  Every
+// expression below is the NumPy expression of the reference matrix class, in its order of
+// operations (1 / d is formed first and then multiplied, never p / d).  These policies use the
+// compact vector set and a small CTA: the per-chain work per metric is a few passes over D
+// elements, so a 256-thread CTA would leave most lanes idle at the D of the hierarchical models.
+// ---------------------------------------------------------------------------------------------
+#ifndef MB200_RM_COMPACT_THREADS
+#define MB200_RM_COMPACT_THREADS 32  // measured against 64 and 128 on C7 (DESIGN.md, K9)
+#endif
+constexpr int RM_COMPACT_THREADS = MB200_RM_COMPACT_THREADS;
+constexpr int RM_COMPACT_MIN_BLOCKS = 65536 / 128 / RM_COMPACT_THREADS;  // <= 128 registers
+
+// diagonal models d(q) and their VJPs w -> sum_i w_i dd_i/dq
+// MB200_RMETRIC_DIAG_QUADRATIC: d_i = a + b q_i^2, vjp(w)_i = 2 b w_i q_i
+struct QuadraticDiagModel {
+  double a, b;
+  int dim;
+  __device__ QuadraticDiagModel(const ModelArgs& m, int d) : a(m.mp[0]), b(m.mp[1]), dim(d) {}
+  __device__ void diag(const Blk& k, const double* q, double* d) const {
+    for (int i = k.tid; i < dim; i += k.nthr) d[i] = a + b * (q[i] * q[i]);
+  }
+  __device__ void vjp(const Blk& k, const double* q, const double* wv, double* out) const {
+    for (int i = k.tid; i < dim; i += k.nthr) out[i] = 2.0 * b * wv[i] * q[i];
+  }
+};
+
+// MB200_RMETRIC_DIAG_FUNNEL_FISHER: expected Fisher information of the funnel,
+// d = [1/9 + (D-1)/2, e^-v, ..., e^-v];  vjp(w) = [-e^-v sum_{i>=1} w_i, 0, ..., 0]
+struct FunnelFisherDiagModel {
+  int dim;
+  __device__ FunnelFisherDiagModel(const ModelArgs&, int d) : dim(d) {}
+  __device__ void diag(const Blk& k, const double* q, double* d) const {
+    const double e = exp(-q[0]);
+    const double d0 = 1.0 / 9.0 + 0.5 * (dim - 1);
+    for (int i = k.tid; i < dim; i += k.nthr) d[i] = (i == 0) ? d0 : e;
+  }
+  __device__ void vjp(const Blk& k, const double* q, const double* wv, double* out) const {
+    double s = 0.0;
+    for (int i = 1 + k.tid; i < dim; i += k.nthr) s += wv[i];
+    s = block_sum(k, s);
+    const double e = exp(-q[0]);
+    for (int i = k.tid; i < dim; i += k.nthr) out[i] = (i == 0) ? -e * s : 0.0;
+  }
+};
+
+template <class Target, class Model>
+struct DiagonalMetric {
+  static constexpr bool SOFTABS = false;
+  static constexpr bool COMPACT = true;
+  static constexpr int N_MATS = 0;
+  static constexpr int MIN_BLOCKS = RM_COMPACT_MIN_BLOCKS;
+  static constexpr int THREADS = RM_COMPACT_THREADS;
+  const Target& t;
+  Model model;
+  __device__ DiagonalMetric(const Target& tt, const ModelArgs& m) : t(tt), model(m, tt.dim) {}
+  __device__ void reset() {}
+
+  // d in w.lam, 1 / d in w.sa; LinAlgError status unless every d_i > 0 (NaN fails), the check
+  // of PositiveDiagonalMatrix (matrices.py:778-780)
+  __device__ int build(const Blk& k, RmWork& w, const double* q) {
+    model.diag(k, q, w.lam);
+    bool bad = false;
+    for (int i = k.tid; i < w.dim; i += k.nthr) {
+      const double d = w.lam[i];
+      w.sa[i] = 1.0 / d;
+      if (!(d > 0.0)) bad = true;
+    }
+    return block_any(k, bad) ? MB200_STATUS_LINALG : 0;
+  }
+  // sum(log |d|)  (SymmetricMatrix.log_abs_det, matrices.py:458-459)
+  __device__ double log_abs_det(const Blk& k, RmWork& w) const {
+    double s = 0.0;
+    for (int i = k.tid; i < w.dim; i += k.nthr) s += log(fabs(w.lam[i]));
+    return block_sum(k, s);
+  }
+  // (1 / d) * v
+  __device__ void inv_matvec(const Blk& k, RmWork& w, const double* v, double* out) const {
+    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = w.sa[i] * v[i];
+    __syncthreads();
+  }
+  // d ** 0.5 * v
+  __device__ bool sqrt_matvec(const Blk& k, RmWork& w, const double* v, double* out) const {
+    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = sqrt(w.lam[i]) * v[i];
+    __syncthreads();
+    return true;
+  }
+  // vjp(grad_log_abs_det) with grad_log_abs_det = 1.0 / d  (matrices.py:758-759)
+  __device__ void vjp_grad_log_abs_det(const Blk& k, RmWork& w, const double* q, double* out) {
+    model.vjp(k, q, w.sa, out);
+    __syncthreads();
+  }
+  // vjp(grad_quadratic_form_inv(p)) with grad_quadratic_form_inv(p) = -((1 / d) * p) ** 2
+  // (matrices.py:761-762)
+  __device__ void vjp_grad_quad_inv(const Blk& k, RmWork& w, const double* q, const double* p,
+                                    double* out) {
+    for (int i = k.tid; i < w.dim; i += k.nthr) {
+      const double x = w.sa[i] * p[i];
+      w.ev[i] = -(x * x);
+    }
+    __syncthreads();  // a model VJP may read entries other threads wrote (funnel: sum over i >= 1)
+    model.vjp(k, q, w.ev, out);
+    __syncthreads();
+  }
+};
+
+template <class Target>
+using QuadraticDiagonalMetric = DiagonalMetric<Target, QuadraticDiagModel>;
+template <class Target>
+using FunnelFisherMetric = DiagonalMetric<Target, FunnelFisherDiagModel>;
+
+// MB200_RMETRIC_SCALAR_QUADRATIC: M(q) = s(q) I with s = a + b |q|^2, vjp(w) = 2 b w q.  The
+// scalar and its reciprocal are block-uniform registers.
+template <class Target>
+struct ScalarMetric {
+  static constexpr bool SOFTABS = false;
+  static constexpr bool COMPACT = true;
+  static constexpr int N_MATS = 0;
+  static constexpr int MIN_BLOCKS = RM_COMPACT_MIN_BLOCKS;
+  static constexpr int THREADS = RM_COMPACT_THREADS;
+  const Target& t;
+  double a, b, s, inv_s;
+  __device__ ScalarMetric(const Target& tt, const ModelArgs& m)
+      : t(tt), a(m.mp[0]), b(m.mp[1]), s(1.0), inv_s(1.0) {}
+  __device__ void reset() {}
+
+  // LinAlgError status unless s > 0 (NaN fails): PositiveScaledIdentityMatrix (matrices.py:692-694)
+  __device__ int build(const Blk& k, RmWork& w, const double* q) {
+    double acc = 0.0;
+    for (int i = k.tid; i < w.dim; i += k.nthr) acc = fma(q[i], q[i], acc);
+    s = a + b * block_sum(k, acc);
+    inv_s = 1.0 / s;
+    return (s > 0.0) ? 0 : MB200_STATUS_LINALG;
+  }
+  // D * log(|s|)  (matrices.py:659-667)
+  __device__ double log_abs_det(const Blk&, RmWork& w) const { return w.dim * log(fabs(s)); }
+  // (1 / s) * v
+  __device__ void inv_matvec(const Blk& k, RmWork& w, const double* v, double* out) const {
+    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = inv_s * v[i];
+    __syncthreads();
+  }
+  // s ** 0.5 * v
+  __device__ bool sqrt_matvec(const Blk& k, RmWork& w, const double* v, double* out) const {
+    const double r = sqrt(s);
+    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = r * v[i];
+    __syncthreads();
+    return true;
+  }
+  // vjp(D / s)  (grad_log_abs_det, matrices.py:669-670)
+  __device__ void vjp_grad_log_abs_det(const Blk& k, RmWork& w, const double* q, double* out) {
+    const double g = w.dim / s;
+    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = 2.0 * b * g * q[i];
+    __syncthreads();
+  }
+  // vjp(-sum(p ** 2) / s ** 2)  (grad_quadratic_form_inv, matrices.py:672-673)
+  __device__ void vjp_grad_quad_inv(const Blk& k, RmWork& w, const double* q, const double* p,
+                                    double* out) {
+    double acc = 0.0;
+    for (int i = k.tid; i < w.dim; i += k.nthr) acc = fma(p[i], p[i], acc);
+    const double g = -block_sum(k, acc) / (s * s);
+    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = 2.0 * b * g * q[i];
+    __syncthreads();
+  }
+};
+
+// ---------------------------------------------------------------------------------------------
 // K4: solve_fixed_point_direct (solvers.py:47-94) for one chain, block-cooperative.
 // `func(x_in, x_out)` returns 0 or a failure code (any failure inside the solver is a
 // ConvergenceError, :89-92).  The same iterate sequence and the same stopping rule as the
@@ -1618,9 +1860,12 @@ __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN
   blk.warp = threadIdx.x >> 5;
   blk.nwarp = blockDim.x >> 5;
   RmWork w;
-  rm_carve(w, smem, dim, n_mats, blk,
-           model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
-                                      : nullptr);
+  if constexpr (rm_compact_policy<MetricT<Target>>::value)
+    rm_carve_compact(w, smem, dim, midpoint, blk);
+  else
+    rm_carve(w, smem, dim, n_mats, blk,
+             model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
+                                        : nullptr);
   const Target target(model, dim);
   // scratch of DENSE_MTP targets: [dim] doubles behind the staging rows in the Vn / z region
   target.attach(w.Vn != nullptr ? w.Vn + (size_t)(blk.nwarp + 1) * dim : nullptr);
@@ -1690,9 +1935,12 @@ __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN
   blk.tid = threadIdx.x, blk.nthr = blockDim.x, blk.lane = threadIdx.x & 31;
   blk.warp = threadIdx.x >> 5, blk.nwarp = blockDim.x >> 5;
   RmWork w;
-  rm_carve(w, smem, dim, n_mats, blk,
-           model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
-                                      : nullptr);
+  if constexpr (rm_compact_policy<MetricT<Target>>::value)
+    rm_carve_compact(w, smem, dim, 0, blk);
+  else
+    rm_carve(w, smem, dim, n_mats, blk,
+             model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
+                                        : nullptr);
   const Target target(model, dim);
   // scratch of DENSE_MTP targets: [dim] doubles behind the staging rows in the Vn / z region
   target.attach(w.Vn != nullptr ? w.Vn + (size_t)(blk.nwarp + 1) * dim : nullptr);
@@ -1725,9 +1973,12 @@ __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN
   blk.tid = threadIdx.x, blk.nthr = blockDim.x, blk.lane = threadIdx.x & 31;
   blk.warp = threadIdx.x >> 5, blk.nwarp = blockDim.x >> 5;
   RmWork w;
-  rm_carve(w, smem, dim, n_mats, blk,
-           model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
-                                      : nullptr);
+  if constexpr (rm_compact_policy<MetricT<Target>>::value)
+    rm_carve_compact(w, smem, dim, 0, blk);
+  else
+    rm_carve(w, smem, dim, n_mats, blk,
+             model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
+                                        : nullptr);
   const Target target(model, dim);
   // scratch of DENSE_MTP targets: [dim] doubles behind the staging rows in the Vn / z region
   target.attach(w.Vn != nullptr ? w.Vn + (size_t)(blk.nwarp + 1) * dim : nullptr);

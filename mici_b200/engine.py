@@ -23,6 +23,12 @@ def build_system(problem):
     if problem.system == "dense_riemannian":
         mm = targets.make_metric_model(problem.metric_model, **problem.metric_params)
         return systems.DenseRiemannianMetricSystem(target, mm)
+    if problem.system == "diagonal_riemannian":
+        mm = targets.make_metric_model(problem.metric_model, **problem.metric_params)
+        return systems.DiagonalRiemannianMetricSystem(target, mm)
+    if problem.system == "scalar_riemannian":
+        mm = targets.make_metric_model(problem.metric_model, **problem.metric_params)
+        return systems.ScalarRiemannianMetricSystem(target, mm)
     raise KeyError(problem.system)
 
 

@@ -23,12 +23,13 @@ class Problem:
         name: config label (``"C0"`` .. ``"C4"``).
         integrator: ``"leapfrog"`` | ``"implicit_leapfrog"`` | ``"constrained_leapfrog"``.
         system: ``"euclidean"`` | ``"softabs_riemannian"`` | ``"dense_riemannian"`` |
-            ``"constrained_euclidean"``.
+            ``"diagonal_riemannian"`` | ``"scalar_riemannian"`` | ``"constrained_euclidean"``.
         target: target-model name (``mici_b200.targets`` registry key).
         target_params: constructor kwargs of the target model.
         metric: ``None`` (identity), 1-D (diagonal) or 2-D (dense SPD) array -- the fixed
             metric of Euclidean systems.
-        metric_model / metric_params: position-dependent metric (dense Riemannian only).
+        metric_model / metric_params: position-dependent metric (dense, diagonal and scalar
+            Riemannian systems).
         step_size: integrator ``step_size``.
         pos, mom: ``[n_chains, dim]`` initial states.
     """
@@ -256,6 +257,50 @@ def c5_dense_hadamard(n_chains=8192, dim=512, seed=BASE_SEED + 7, coeff=0.1,
     )
 
 
+def funnel_fisher_diagonal(q):
+    """The funnel's expected Fisher information d(q) = [1/9 + (D-1)/2, e^-v, ..., e^-v] for a
+    batch ``q`` [n, D] (the metric of ``mici_b200.targets.FunnelFisherMetric``)."""
+    d = np.empty_like(q)
+    d[:, 0] = 1.0 / 9.0 + 0.5 * (q.shape[1] - 1)
+    d[:, 1:] = np.exp(-q[:, :1])
+    return d
+
+
+def c7_funnel_riemannian(n_chains=8192, dim=128, seed=BASE_SEED + 10, metric_kind="fisher",
+                         integrator="implicit_leapfrog"):
+    """The funnel of C1 on a Riemannian system with an O(D) position-dependent metric:
+    ``metric_kind="fisher"`` -- ``DiagonalRiemannianMetricSystem`` with the funnel's expected
+    Fisher information; ``"scalar"`` -- ``ScalarRiemannianMetricSystem`` with s = 1 + |q|^2 / D.
+    Momenta are drawn from N(0, M(q)) at the initial positions.  Step sizes chosen on the CPU
+    oracle (10 steps): Fisher 0.2 -- all of the first 256 chains complete, median |h error| 1.9;
+    scalar 0.05 -- all of the first 64 complete, median |h error| 0.8 (at 0.1 the median error is
+    250 and at 0.2 only 84 % complete: one scale for all coordinates cannot follow the funnel's
+    neck)."""
+    rng = np.random.default_rng(seed)
+    pos = 0.5 * rng.standard_normal((n_chains, dim))
+    z = rng.standard_normal((n_chains, dim))
+    if metric_kind == "fisher":
+        system, model, params = "diagonal_riemannian", "funnel_fisher", {}
+        mom = z * np.sqrt(funnel_fisher_diagonal(pos))
+    elif metric_kind == "scalar":
+        system, model, params = "scalar_riemannian", "scalar_quadratic", {"a": 1.0, "b": 1.0 / dim}
+        mom = z * np.sqrt(1.0 + (pos * pos).sum(1) / dim)[:, None]
+    else:
+        raise ValueError(metric_kind)
+    return Problem(
+        name="C7",
+        integrator=integrator,
+        system=system,
+        target="neal_funnel",
+        target_params={"dim": dim},
+        step_size=0.2 if metric_kind == "fisher" else 0.05,
+        pos=pos,
+        mom=mom,
+        metric_model=model,
+        metric_params=params,
+    )
+
+
 def sphere_constrained(n_chains=64, dim=10, seed=BASE_SEED + 5, metric_kind="dense",
                        dens_wrt_hausdorff=True):
     """Extra parity case for K6 beyond C3: unit sphere in R^dim, tilted Gaussian density,
@@ -347,6 +392,7 @@ CONFIGS = {
     "C4": c4_dense_riemannian,
     "C5": c5_dense_hadamard,
     "C6": c6_softabs_quartic,
+    "C7": c7_funnel_riemannian,
     "S1": sphere_constrained,
     "S2": multi_sphere_constrained,
     "G1": g1_gaussian_split,

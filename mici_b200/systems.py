@@ -6,6 +6,8 @@ hot path:
 * ``DenseConstrainedEuclideanMetricSystem``   systems.py:619-873, 876-1031
 * ``DenseRiemannianMetricSystem``             systems.py:1187-1402, 1710-1760
 * ``SoftAbsRiemannianMetricSystem``           systems.py:1763-1920
+* ``ScalarRiemannianMetricSystem``            systems.py:1405-1490
+* ``DiagonalRiemannianMetricSystem``          systems.py:1493-1571
 
 Differences forced by the device: ``neg_log_dens`` is an instance of
 ``mici_b200.targets.Target`` (a model compiled into the library) instead of a Python callable,
@@ -23,7 +25,16 @@ import torch
 
 from . import _lib
 from .errors import LinAlgError
-from .targets import RMETRIC_SOFTABS, HadamardMetric, Rank1Metric, Target
+from .targets import (
+    RMETRIC_SOFTABS,
+    FunnelFisherMetric,
+    HadamardMetric,
+    NealFunnel,
+    QuadraticDiagonalMetric,
+    QuadraticScalarMetric,
+    Rank1Metric,
+    Target,
+)
 
 METRIC_IDENTITY, METRIC_DIAGONAL, METRIC_DENSE = 0, 1, 2
 
@@ -611,3 +622,52 @@ class SoftAbsRiemannianMetricSystem(RiemannianMetricSystem):
         self.softabs_coeff = float(softabs_coeff)
         self._rmetric_id = RMETRIC_SOFTABS
         self._rmetric_params = (self.softabs_coeff,)
+
+
+class ScalarRiemannianMetricSystem(RiemannianMetricSystem):
+    """Scaled-identity position-dependent metric ``s(q) I`` (systems.py:1405-1490) with
+    ``PositiveScaledIdentityMatrix`` arithmetic (matrices.py:595-706): ``metric_scalar_func`` is a
+    registered metric model, ``mici_b200.targets.QuadraticScalarMetric`` (s = a + b |q|^2).
+
+    A chain whose ``s(q)`` is not positive fails with status 3 (``LinAlgError``) outside a
+    fixed-point solve and with ``ConvergenceError`` inside one; the reference raises
+    ``ValueError`` in the first case (DESIGN.md section 1)."""
+
+    def __init__(self, neg_log_dens, metric_scalar_func, *, vjp_metric_scalar_func=None,
+                 grad_neg_log_dens=None, backend=None):
+        super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
+        if not isinstance(metric_scalar_func, QuadraticScalarMetric):
+            raise TypeError("`metric_scalar_func` must be a registered metric model "
+                            "(QuadraticScalarMetric).")
+        if vjp_metric_scalar_func is not None:
+            raise ValueError("The metric VJP is fused into the kernels.")
+        self.metric_model = metric_scalar_func
+        self._rmetric_id = metric_scalar_func.rmetric_id
+        self._rmetric_params = metric_scalar_func.params
+
+
+class DiagonalRiemannianMetricSystem(RiemannianMetricSystem):
+    """Diagonal position-dependent metric ``diag(d(q))`` (systems.py:1493-1571) with
+    ``PositiveDiagonalMatrix`` arithmetic (matrices.py:709-792): ``metric_diagonal_func`` is a
+    registered metric model -- ``mici_b200.targets.QuadraticDiagonalMetric`` (d_i = a + b q_i^2)
+    or ``mici_b200.targets.FunnelFisherMetric`` (the funnel's expected Fisher information, funnel
+    target only).  O(D) per metric: a chain's whole state lives in a small CTA's shared memory.
+
+    A chain whose ``d(q)`` has an entry that is not positive fails with status 3
+    (``LinAlgError``) outside a fixed-point solve and with ``ConvergenceError`` inside one; the
+    reference raises ``ValueError`` in the first case (DESIGN.md section 1)."""
+
+    def __init__(self, neg_log_dens, metric_diagonal_func, *, vjp_metric_diagonal_func=None,
+                 grad_neg_log_dens=None, backend=None):
+        super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
+        if not isinstance(metric_diagonal_func, (QuadraticDiagonalMetric, FunnelFisherMetric)):
+            raise TypeError("`metric_diagonal_func` must be a registered metric model "
+                            "(QuadraticDiagonalMetric or FunnelFisherMetric).")
+        if isinstance(metric_diagonal_func, FunnelFisherMetric) and not isinstance(
+                neg_log_dens, NealFunnel):
+            raise TypeError("FunnelFisherMetric is the metric of the NealFunnel target.")
+        if vjp_metric_diagonal_func is not None:
+            raise ValueError("The metric VJP is fused into the kernels.")
+        self.metric_model = metric_diagonal_func
+        self._rmetric_id = metric_diagonal_func.rmetric_id
+        self._rmetric_params = metric_diagonal_func.params

@@ -23,6 +23,9 @@ TARGET_QUARTIC = 7
 RMETRIC_SOFTABS = 0
 RMETRIC_RANK1 = 1
 RMETRIC_HADAMARD = 2
+RMETRIC_DIAG_QUADRATIC = 3
+RMETRIC_DIAG_FUNNEL_FISHER = 4
+RMETRIC_SCALAR_QUADRATIC = 5
 
 
 class Target:
@@ -184,11 +187,57 @@ class HadamardMetric:
         self.params = (float(coeff), 0.0, 0.0, 1.0 if generic_rank1_vjp else 0.0)
 
 
+class QuadraticDiagonalMetric:
+    """Position-dependent diagonal metric d_i(q) = a + b q_i^2 (``a > 0``, ``b >= 0``); with
+    ``a = b = 1`` the metric ``1 + q**2`` of the reference's own integrator tests."""
+
+    rmetric_id = RMETRIC_DIAG_QUADRATIC
+    name = "diag_quadratic"
+    aux = None
+
+    def __init__(self, a=1.0, b=1.0):
+        a, b = float(a), float(b)
+        if not (a > 0 and b >= 0):
+            raise ValueError("QuadraticDiagonalMetric needs a > 0 and b >= 0.")
+        self.a, self.b = a, b
+        self.params = (a, b)
+
+
+class FunnelFisherMetric:
+    """Diagonal metric of the funnel (``NealFunnel``): its expected Fisher information
+    d(q) = [1/9 + (D-1)/2, e^-v, ..., e^-v] with v = q[0]."""
+
+    rmetric_id = RMETRIC_DIAG_FUNNEL_FISHER
+    name = "funnel_fisher"
+    aux = None
+    params = ()
+
+
+class QuadraticScalarMetric:
+    """Position-dependent scaled-identity metric s(q) I with s = a + b |q|^2 (``a > 0``,
+    ``b >= 0``)."""
+
+    rmetric_id = RMETRIC_SCALAR_QUADRATIC
+    name = "scalar_quadratic"
+    aux = None
+
+    def __init__(self, a=1.0, b=1.0):
+        a, b = float(a), float(b)
+        if not (a > 0 and b >= 0):
+            raise ValueError("QuadraticScalarMetric needs a > 0 and b >= 0.")
+        self.a, self.b = a, b
+        self.params = (a, b)
+
+
 REGISTRY = {
     cls.name: cls
     for cls in (StdGaussian, NealFunnel, Banana, Quadratic, Quartic, Torus, Sphere, MultiSphere)
 }
-METRIC_REGISTRY = {"rank1": Rank1Metric, "hadamard": HadamardMetric}
+METRIC_REGISTRY = {
+    cls.name: cls
+    for cls in (Rank1Metric, HadamardMetric, QuadraticDiagonalMetric, FunnelFisherMetric,
+                QuadraticScalarMetric)
+}
 
 
 def make_target(name, **params):
