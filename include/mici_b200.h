@@ -82,6 +82,9 @@ extern "C" {
 #define MB200_RMETRIC_DIAG_QUADRATIC 3     /* diagonal d_i = a + b q_i^2;  params: a > 0, b >= 0 */
 #define MB200_RMETRIC_DIAG_FUNNEL_FISHER 4 /* diagonal d = [1/9 + (D-1)/2, e^-v, ..., e^-v], v = q[0]: the funnel's expected Fisher information */
 #define MB200_RMETRIC_SCALAR_QUADRATIC 5   /* scaled identity s I, s = a + b |q|^2;  params: a > 0, b >= 0 */
+/* Cholesky-factored metric M = L L^T given by its lower factor (CholeskyFactoredRiemannianMetricSystem,
+ * systems.py:1574-1653); targets: std-Gaussian, banana, funnel, quadratic */
+#define MB200_RMETRIC_CHOL_QUADRATIC 6 /* L(q) = L0 + c tril(q q^T);  aux: L0 [dim*dim] row-major, upper triangle zero (never read), params: c */
 
 /* fixed-point solvers fused into the implicit integrators (solvers.py:47-94, 97-154) */
 #define MB200_FP_SOLVER_DIRECT 0

@@ -23,13 +23,15 @@ static int launch_implicit(const double* q_in, const double* p_in, double* q_out
   if (compact && smem > 227 * 1024)
     return fail(MB200_ERR_UNSUPPORTED, "dim %d: per-chain vectors (%zu bytes) exceed shared memory",
                 dim, smem);
+  constexpr int ws_mats = rm_workspace_mats<MetricT<Target>>::value;
   if (smem > 227 * 1024) {
-    // SoftAbs beyond shared memory: the same kernels with the matrices in a per-CTA global
-    // workspace (L2-resident operands: slower, but the reference has no dimension limit)
-    if (!MetricT<Target>::SOFTABS)
+    // SoftAbs and Cholesky-factored metrics beyond shared memory: the same kernels with the
+    // matrices in a per-CTA global workspace (L2-resident operands: slower, but the reference
+    // has no dimension limit)
+    if (ws_mats == 0)
       return fail(MB200_ERR_UNSUPPORTED,
                   "dim %d: per-chain metric (%zu bytes) exceeds shared memory", dim, smem);
-    n_mats = RM_NMATS_IN_WORKSPACE + 3;
+    n_mats = RM_NMATS_IN_WORKSPACE + ws_mats;
     smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
     in_ws = true;
     if (smem > 227 * 1024) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
@@ -43,10 +45,10 @@ static int launch_implicit(const double* q_in, const double* p_in, double* q_out
   int64_t blocks = (int64_t)num_sms() * per_sm;
   if (blocks > n) blocks = n;
   ModelArgs margs = m;
-  const size_t per_cta = 3 * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
+  const size_t per_cta = ws_mats * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
   DgScratch scratch(nullptr, 0, in_ws ? per_cta * blocks * sizeof(double) : 0, st);
   if (in_ws) {
-    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "SoftAbs workspace allocation failed");
+    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "metric workspace allocation failed");
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
@@ -105,6 +107,27 @@ static int compact_dispatch(const ModelArgs& m, int dim, const L& l) {
                   : l.template run<QuadraticRTarget, ScalarMetric>();
     default:
       return fail(MB200_ERR_UNSUPPORTED, "target %d not available with diagonal / scalar metrics",
+                  m.target_id);
+  }
+}
+
+// Target / metric pairs of the Cholesky-factored metric (same targets and argument checks as
+// compact_dispatch); `L` as there
+template <class L>
+static int chol_dispatch(const ModelArgs& m, int dim, const L& l) {
+  if (!m.maux)
+    return fail(MB200_ERR_INVALID_ARG, "Cholesky-factored metric needs its base factor (rmetric_aux)");
+  if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
+    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
+  if (m.target_id == MB200_TARGET_QUADRATIC && !m.taux)
+    return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
+  switch (m.target_id) {
+    case MB200_TARGET_STD_GAUSSIAN: return l.template run<StdGaussianRTarget, QuadraticCholeskyMetric>();
+    case MB200_TARGET_BANANA: return l.template run<BananaRTarget, QuadraticCholeskyMetric>();
+    case MB200_TARGET_NEAL_FUNNEL: return l.template run<FunnelRTarget, QuadraticCholeskyMetric>();
+    case MB200_TARGET_QUADRATIC: return l.template run<QuadraticRTarget, QuadraticCholeskyMetric>();
+    default:
+      return fail(MB200_ERR_UNSUPPORTED, "target %d not available with a Cholesky-factored metric",
                   m.target_id);
   }
 }
@@ -197,6 +220,10 @@ static int implicit_dispatch(const double* q_in, const double* p_in, double* q_o
                                                    n_steps, m, fp_tol, fp_div, fp_max, rev_tol,
                                                    h_out, status, n_done, fp_iters, st, midpoint,
                                                    fp_solver});
+  if (m.rmetric_id == MB200_RMETRIC_CHOL_QUADRATIC)
+    return chol_dispatch(m, dim, ImplicitLaunch{q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps,
+                                                m, fp_tol, fp_div, fp_max, rev_tol, h_out, status,
+                                                n_done, fp_iters, st, midpoint, fp_solver});
   return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
 }
 
@@ -208,9 +235,10 @@ static int launch_sample_momentum(const double* q, const double* z, double* p_ou
   constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
   size_t smem = (compact ? rm_compact_doubles(dim, 0) : rm_smem_doubles(dim, n_mats)) * sizeof(double);
   bool in_ws = false;
+  constexpr int ws_mats = rm_workspace_mats<MetricT<Target>>::value;
   if (smem > 227 * 1024) {
-    if (!MetricT<Target>::SOFTABS) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
-    n_mats = RM_NMATS_IN_WORKSPACE + 3;
+    if (ws_mats == 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
+    n_mats = RM_NMATS_IN_WORKSPACE + ws_mats;
     smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
     in_ws = true;
     if (smem > 227 * 1024) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
@@ -225,10 +253,10 @@ static int launch_sample_momentum(const double* q, const double* z, double* p_ou
   }
   if (blocks > n) blocks = n;
   ModelArgs margs = m;
-  const size_t per_cta = 3 * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
+  const size_t per_cta = ws_mats * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
   DgScratch scratch(nullptr, 0, in_ws ? per_cta * blocks * sizeof(double) : 0, st);
   if (in_ws) {
-    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "SoftAbs workspace allocation failed");
+    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "metric workspace allocation failed");
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
@@ -245,9 +273,10 @@ static int launch_velocity(const double* q, const double* p, double* vel, int64_
   constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
   size_t smem = (compact ? rm_compact_doubles(dim, 0) : rm_smem_doubles(dim, n_mats)) * sizeof(double);
   bool in_ws = false;
+  constexpr int ws_mats = rm_workspace_mats<MetricT<Target>>::value;
   if (smem > 227 * 1024) {
-    if (!MetricT<Target>::SOFTABS) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
-    n_mats = RM_NMATS_IN_WORKSPACE + 3;
+    if (ws_mats == 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
+    n_mats = RM_NMATS_IN_WORKSPACE + ws_mats;
     smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
     in_ws = true;
     if (smem > 227 * 1024) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
@@ -262,10 +291,10 @@ static int launch_velocity(const double* q, const double* p, double* vel, int64_
   }
   if (blocks > n) blocks = n;
   ModelArgs margs = m;
-  const size_t per_cta = 3 * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
+  const size_t per_cta = ws_mats * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
   DgScratch scratch(nullptr, 0, in_ws ? per_cta * blocks * sizeof(double) : 0, st);
   if (in_ws) {
-    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "SoftAbs workspace allocation failed");
+    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "metric workspace allocation failed");
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
@@ -429,6 +458,9 @@ int mb200_sample_momentum_riemannian(const double* pos, const double* normals, d
   if (is_compact_rmetric(m.rmetric_id))
     return compact_dispatch(m, dim, VectorLaunch{pos, normals, mom_out, n_chains, dim, m, status,
                                                  st, false});
+  if (m.rmetric_id == MB200_RMETRIC_CHOL_QUADRATIC)
+    return chol_dispatch(m, dim, VectorLaunch{pos, normals, mom_out, n_chains, dim, m, status, st,
+                                              false});
   return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
 }
 
@@ -470,6 +502,8 @@ int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_o
   if (is_compact_rmetric(m.rmetric_id))
     return compact_dispatch(m, dim, VectorLaunch{pos, mom, vel_out, n_chains, dim, m, status, st,
                                                  true});
+  if (m.rmetric_id == MB200_RMETRIC_CHOL_QUADRATIC)
+    return chol_dispatch(m, dim, VectorLaunch{pos, mom, vel_out, n_chains, dim, m, status, st, true});
   return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
 }
 

@@ -385,7 +385,8 @@ constexpr int RM_NMATS_GLOBAL = -1;  // n_mats code: compact vector set + dg_sme
 // n_mats code RM_NMATS_IN_WORKSPACE + k: the k per-chain D x D matrices of the shared-memory
 // policies (SoftAbs: eigenvectors, work / divided-difference matrix, warm-start matrix) live in
 // the per-CTA GLOBAL workspace instead (dimensions whose matrices exceed 227 KB: SoftAbs at
-// D > ~100); the algorithms are unchanged, the operands are simply L2-resident
+// D > ~100, the Cholesky-factored metric's factor at D > ~150); the algorithms are unchanged,
+// the operands are simply L2-resident
 constexpr int RM_NMATS_IN_WORKSPACE = 100;
 
 // n_mats: per-chain D x D matrices kept in shared memory (SoftAbs 2, or 3 with warm-started
@@ -519,6 +520,30 @@ struct rm_compact_policy {
 template <class M>
 struct rm_compact_policy<M, decltype(void(M::COMPACT))> {
   static constexpr bool value = M::COMPACT;
+};
+
+// number of per-chain D x D matrices a policy keeps in the per-CTA global workspace
+// (n_mats = RM_NMATS_IN_WORKSPACE + value) when its shared-memory layout does not fit: policies
+// that declare `static constexpr int WORKSPACE_MATS`; 0 (no such route) for the others
+template <class M, class = void>
+struct rm_workspace_mats {
+  static constexpr int value = 0;
+};
+template <class M>
+struct rm_workspace_mats<M, decltype(void(M::WORKSPACE_MATS))> {
+  static constexpr int value = M::WORKSPACE_MATS;
+};
+
+// true for policies whose build() accepts a metric that cannot be solved with (a zero pivot of
+// a triangular factor: `static constexpr bool CAN_BE_SINGULAR = true` and a `singular()`
+// member); the velocity kernel and the energy then report it
+template <class M, class = void>
+struct rm_singular_policy {
+  static constexpr bool value = false;
+};
+template <class M>
+struct rm_singular_policy<M, decltype(void(M::CAN_BE_SINGULAR))> {
+  static constexpr bool value = M::CAN_BE_SINGULAR;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -912,10 +937,12 @@ __device__ inline bool cholesky_inplace(const Blk& k, double* M, int n, int ld) 
   return true;
 }
 
-// x = (L L^T)^-1 b by forward / back substitution (scipy solve_triangular, matrices.py:897-912).
-// Column-oriented so that each elimination step is parallel over rows.  x may alias b.
-__device__ inline void cholesky_solve(const Blk& k, const double* L, int n, int ld,
-                                      const double* b, double* x) {
+// Forward / back substitution with a lower factor L (scipy solve_triangular, matrices.py:897-912).
+// Column-oriented so that each elimination step is parallel over rows.  The two halves are also
+// used on their own (the Cholesky-factored metric needs L^-1 b).
+// x = L^-1 b (forward substitution); x may alias b
+__device__ __forceinline__ void cholesky_forward(const Blk& k, const double* L, int n, int ld,
+                                                 const double* b, double* x) {
   for (int i = k.tid; i < n; i += k.nthr) x[i] = b[i];
   __syncthreads();
   for (int j = 0; j < n; ++j) {  // L y = b
@@ -925,6 +952,10 @@ __device__ inline void cholesky_solve(const Blk& k, const double* L, int n, int 
     for (int i = j + 1 + k.tid; i < n; i += k.nthr) x[i] -= L[i * ld + j] * xj;
     __syncthreads();
   }
+}
+// x <- L^-T x in place (back substitution)
+__device__ __forceinline__ void cholesky_back(const Blk& k, const double* L, int n, int ld,
+                                              double* x) {
   for (int j = n - 1; j >= 0; --j) {  // L^T x = y
     if (k.tid == 0) x[j] /= L[j * ld + j];
     __syncthreads();
@@ -932,6 +963,12 @@ __device__ inline void cholesky_solve(const Blk& k, const double* L, int n, int 
     for (int i = k.tid; i < j; i += k.nthr) x[i] -= L[j * ld + i] * xj;
     __syncthreads();
   }
+}
+// x = (L L^T)^-1 b; x may alias b
+__device__ inline void cholesky_solve(const Blk& k, const double* L, int n, int ld,
+                                      const double* b, double* x) {
+  cholesky_forward(k, L, n, ld, b, x);
+  cholesky_back(k, L, n, ld, x);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -944,6 +981,8 @@ template <class Target>
 struct SoftAbsMetric {
   static constexpr bool SOFTABS = true;
   static constexpr int N_MATS = 2;
+  // beyond shared memory: eigenvectors, work / divided-difference and warm-start matrices
+  static constexpr int WORKSPACE_MATS = 3;
   // register budget: two CTAs per SM (<= 128 registers); stated explicitly because ptxas's own
   // choice flips with unrelated code changes (48 vs 80 registers measured 3.4x apart on C4)
   static constexpr int MIN_BLOCKS = 2;
@@ -1504,6 +1543,154 @@ struct ScalarMetric {
 };
 
 // ---------------------------------------------------------------------------------------------
+// K10: CholeskyFactoredRiemannianMetricSystem (systems.py:1574-1653): the metric is given by its
+// lower-triangular factor L(q), M = L L^T, with TriangularFactoredPositiveDefiniteMatrix
+// arithmetic (matrices.py:795-1114): no factorisation, O(D^2) per metric.
+// ---------------------------------------------------------------------------------------------
+#ifndef MB200_RM_CHOL_THREADS
+#define MB200_RM_CHOL_THREADS 256  // measured against 64 and 128 on C8 (DESIGN.md, K10)
+#endif
+
+// Inclusive prefix sums P_k = sum_{j<=k} b_j q_j and inclusive suffix sums S_k = sum_{i>=k} a_i q_i
+// over the CTA, a tile of nthr elements at a time (warp shuffles, warp totals in k.red[0..8) and
+// k.red[16..24): at most 256 threads).  P and S must not alias a, b or q.
+__device__ inline void block_prefix_suffix(const Blk& k, int n, const double* a, const double* b,
+                                           const double* q, double* P, double* S) {
+  double carry_p = 0.0, carry_s = 0.0;
+  for (int base = 0; base < n; base += k.nthr) {
+    const int i = base + k.tid;  // prefix element of this thread
+    const int r = n - 1 - i;     // suffix element of this thread (descending)
+    double x = i < n ? b[i] * q[i] : 0.0;
+    double y = i < n ? a[r] * q[r] : 0.0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const double xo = __shfl_up_sync(FULL_MASK, x, o), yo = __shfl_up_sync(FULL_MASK, y, o);
+      if (k.lane >= o) x += xo, y += yo;
+    }
+    __syncthreads();  // the previous tile's (or a block reduction's) readers of k.red are done
+    if (k.lane == 31) k.red[k.warp] = x, k.red[16 + k.warp] = y;
+    __syncthreads();
+    double px = carry_p, py = carry_s;
+    for (int v = 0; v < k.warp; ++v) px += k.red[v], py += k.red[16 + v];
+    if (i < n) P[i] = px + x, S[r] = py + y;
+    for (int v = 0; v < k.nwarp; ++v) carry_p += k.red[v], carry_s += k.red[16 + v];
+  }
+  __syncthreads();
+}
+
+// MB200_RMETRIC_CHOL_QUADRATIC: L(q) = L0 + c tril(q q^T), L0 = aux [D x D] row-major lower
+// triangular (the host zeroes its upper triangle; it is never read here).  VJPs of the two
+// structured lower-triangular arguments the policy produces, sum_ij V_ij dL_ij/dq_k with
+// dL_ij/dq_k = c (delta_ik q_j + q_i delta_jk), j <= i -- V is never formed:
+//   V = diag(d)          ->  c (d_k q_k + d_k q_k)
+//   V = tril(s a b^T)    ->  c s (a_k sum_{j<=k} b_j q_j + b_k sum_{i>=k} a_i q_i)
+struct QuadraticCholModel {
+  const double* L0;
+  double c;
+  int dim;
+  __device__ QuadraticCholModel(const ModelArgs& m, int d) : L0(m.maux), c(m.mp[0]), dim(d) {}
+  // lower triangle of L(q) into L (stride ld); true iff every entry written is finite
+  __device__ bool fill(const Blk& k, const double* q, double* L, int ld) const {
+    bool bad = false;
+    for (int idx = k.tid; idx < dim * dim; idx += k.nthr) {
+      const int i = idx / dim, j = idx - i * dim;
+      if (j > i) continue;
+      const double v = L0[idx] + c * (q[i] * q[j]);
+      if (!isfinite(v)) bad = true;
+      L[i * ld + j] = v;
+    }
+    return !bad;
+  }
+  __device__ void vjp_diag(const Blk& k, const double* q, const double* d, double* out) const {
+    for (int i = k.tid; i < dim; i += k.nthr) {
+      const double x = d[i] * q[i];
+      out[i] = c * (x + x);
+    }
+  }
+  // P, S: [dim] shared scratch for the scans
+  __device__ void vjp_outer(const Blk& k, const double* q, double s, const double* a,
+                            const double* b, double* P, double* S, double* out) const {
+    block_prefix_suffix(k, dim, a, b, q, P, S);
+    for (int i = k.tid; i < dim; i += k.nthr)
+      out[i] = c * (s * (a[i] * P[i] + b[i] * S[i]));
+  }
+};
+
+// TriangularFactoredPositiveDefiniteMatrix(L, factor_is_lower=True):
+//   log|M| = 2 sum log|L_ii|                          (matrices.py:982-984, 850-852)
+//   M^-1 v = L^-T (L^-1 v), no inverse formed          (:1110-1111, 897-912)
+//   sqrt(M) z = L z                                     (:1113-1114)
+//   grad_log_abs_det = diag(2 / diag L)                 (:1048-1050)
+//   grad_quadratic_form_inv(p) = tril(-2 (M^-1 p)(L^-1 p)^T)   (:1052-1058)
+// build() fails (LinAlgError status) only for a non-finite entry of the lower triangle
+// (ExplicitArrayMatrix, :207-215); a zero or negative diagonal entry is accepted, as by the
+// reference: a zero pivot surfaces through IEEE arithmetic in the solves (-> ConvergenceError
+// inside a fixed-point solve) and through singular() in the velocity and energy evaluations.
+template <class Target, class Model>
+struct CholeskyFactoredMetric {
+  static constexpr bool SOFTABS = false;
+  static constexpr bool CAN_BE_SINGULAR = true;
+  static constexpr int N_MATS = 1;          // the factor [dim x (dim + 1)]
+  static constexpr int WORKSPACE_MATS = 1;  // ... in the per-CTA global workspace beyond ~150
+  static constexpr int THREADS = MB200_RM_CHOL_THREADS;
+  static constexpr int MIN_BLOCKS = 65536 / 128 / THREADS;  // <= 128 registers
+  const Target& t;
+  Model model;
+  __device__ CholeskyFactoredMetric(const Target& tt, const ModelArgs& m) : t(tt), model(m, tt.dim) {}
+  __device__ void reset() {}
+
+  __device__ int build(const Blk& k, RmWork& w, const double* q) {
+    const bool ok = model.fill(k, q, w.M1, w.ld);
+    return block_any(k, !ok) ? MB200_STATUS_LINALG : 0;  // "Array is not finite" (:207-215)
+  }
+  // a zero diagonal entry: scipy's solve_triangular raises LinAlgError ("singular matrix")
+  __device__ bool singular(const Blk& k, RmWork& w) const {
+    bool z = false;
+    for (int i = k.tid; i < w.dim; i += k.nthr)
+      if (w.M1[i * w.ld + i] == 0.0) z = true;
+    return block_any(k, z);
+  }
+  __device__ double log_abs_det(const Blk& k, RmWork& w) const {
+    double s = 0.0;
+    for (int i = k.tid; i < w.dim; i += k.nthr) s += log(fabs(w.M1[i * w.ld + i]));
+    return 2.0 * block_sum(k, s);
+  }
+  __device__ void inv_matvec(const Blk& k, RmWork& w, const double* v, double* out) const {
+    cholesky_solve(k, w.M1, w.dim, w.ld, v, out);
+  }
+  __device__ bool sqrt_matvec(const Blk& k, RmWork& w, const double* v, double* out) const {
+    for (int i = k.tid; i < w.dim; i += k.nthr) {
+      double s = 0.0;
+      for (int j = 0; j <= i; ++j) s = fma(w.M1[i * w.ld + j], v[j], s);
+      out[i] = s;
+    }
+    __syncthreads();
+    return true;
+  }
+  // d = 2 / diag L in w.ev
+  __device__ void vjp_grad_log_abs_det(const Blk& k, RmWork& w, const double* q, double* out) {
+    for (int i = k.tid; i < w.dim; i += k.nthr) w.ev[i] = 2.0 / w.M1[i * w.ld + i];
+    __syncthreads();
+    model.vjp_diag(k, q, w.ev, out);
+    __syncthreads();
+  }
+  // b = L^-1 p in w.lam (computed once: M^-1 p = L^-T b continues from it), a = M^-1 p in w.ev;
+  // scan scratch w.sa, w.gsa
+  __device__ void vjp_grad_quad_inv(const Blk& k, RmWork& w, const double* q, const double* p,
+                                    double* out) {
+    cholesky_forward(k, w.M1, w.dim, w.ld, p, w.lam);
+    for (int i = k.tid; i < w.dim; i += k.nthr) w.ev[i] = w.lam[i];
+    __syncthreads();
+    cholesky_back(k, w.M1, w.dim, w.ld, w.ev);
+    model.vjp_outer(k, q, -2.0, w.ev, w.lam, w.sa, w.gsa, out);
+    __syncthreads();
+  }
+};
+
+template <class Target>
+using QuadraticCholeskyMetric = CholeskyFactoredMetric<Target, QuadraticCholModel>;
+
+// ---------------------------------------------------------------------------------------------
 // K4: solve_fixed_point_direct (solvers.py:47-94) for one chain, block-cooperative.
 // `func(x_in, x_out)` returns 0 or a failure code (any failure inside the solver is a
 // ConvergenceError, :89-92).  The same iterate sequence and the same stopping rule as the
@@ -1833,6 +2020,8 @@ struct ImplicitLeapfrog {
   __device__ double hamiltonian() {
     m.reset();
     if (m.build(k, w, w.q) != 0) return nan("");  // diagnostics: not counted
+    if constexpr (rm_singular_policy<Metric>::value)
+      if (m.singular(k, w)) return nan("");
     m.inv_matvec(k, w, w.p, w.v1);
     double s = 0.0;
     for (int i = k.tid; i < w.dim; i += k.nthr) s = fma(w.p[i], w.v1[i], s);
@@ -1991,7 +2180,9 @@ __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN
     }
     __syncthreads();
     metric.reset();
-    const int st = metric.build(blk, w, w.q) != 0 ? MB200_STATUS_LINALG : MB200_STATUS_OK;
+    int st = metric.build(blk, w, w.q) != 0 ? MB200_STATUS_LINALG : MB200_STATUS_OK;
+    if constexpr (rm_singular_policy<MetricT<Target>>::value)
+      if (st == MB200_STATUS_OK && metric.singular(blk, w)) st = MB200_STATUS_LINALG;
     if (st == MB200_STATUS_OK) metric.inv_matvec(blk, w, w.p, w.v1);
     for (int i = blk.tid; i < dim; i += blk.nthr)
       vel_out[(size_t)ch * dim + i] = (st == MB200_STATUS_OK) ? w.v1[i] : nan("");

@@ -29,6 +29,9 @@ def build_system(problem):
     if problem.system == "scalar_riemannian":
         mm = targets.make_metric_model(problem.metric_model, **problem.metric_params)
         return systems.ScalarRiemannianMetricSystem(target, mm)
+    if problem.system == "cholesky_riemannian":
+        mm = targets.make_metric_model(problem.metric_model, **problem.metric_params)
+        return systems.CholeskyFactoredRiemannianMetricSystem(target, mm)
     raise KeyError(problem.system)
 
 

@@ -23,13 +23,14 @@ class Problem:
         name: config label (``"C0"`` .. ``"C4"``).
         integrator: ``"leapfrog"`` | ``"implicit_leapfrog"`` | ``"constrained_leapfrog"``.
         system: ``"euclidean"`` | ``"softabs_riemannian"`` | ``"dense_riemannian"`` |
-            ``"diagonal_riemannian"`` | ``"scalar_riemannian"`` | ``"constrained_euclidean"``.
+            ``"diagonal_riemannian"`` | ``"scalar_riemannian"`` | ``"cholesky_riemannian"`` |
+            ``"constrained_euclidean"``.
         target: target-model name (``mici_b200.targets`` registry key).
         target_params: constructor kwargs of the target model.
         metric: ``None`` (identity), 1-D (diagonal) or 2-D (dense SPD) array -- the fixed
             metric of Euclidean systems.
-        metric_model / metric_params: position-dependent metric (dense, diagonal and scalar
-            Riemannian systems).
+        metric_model / metric_params: position-dependent metric (dense, diagonal, scalar and
+            Cholesky-factored Riemannian systems).
         step_size: integrator ``step_size``.
         pos, mom: ``[n_chains, dim]`` initial states.
     """
@@ -301,6 +302,44 @@ def c7_funnel_riemannian(n_chains=8192, dim=128, seed=BASE_SEED + 10, metric_kin
     )
 
 
+def chol_quadratic_factor(pos, base_factor, coeff):
+    """L(q) = L0 + c tril(q q^T) for a batch ``pos`` [n, D] (the factor of
+    ``mici_b200.targets.QuadraticCholeskyMetric``), [n, D, D]."""
+    return base_factor + coeff * np.tril(pos[:, :, None] * pos[:, None, :])
+
+
+def c8_cholesky_riemannian(n_chains=8192, dim=128, seed=BASE_SEED + 11, coeff=None,
+                           integrator="implicit_leapfrog", step_size=0.1):
+    """``CholeskyFactoredRiemannianMetricSystem`` on the quadratic target of C4 (precision
+    P = I + 0.1 G G^T / D, generated the same way): L(q) = chol(P) + c tril(q q^T) with
+    c = 1/D, so M(0) = P, the target's Fisher information.  Momenta are drawn from N(0, M(q))
+    at the initial positions (p = L(q) z).  Step size chosen on the CPU oracle (10 steps, first
+    64 chains, every chain completing at each size): 0.1 -- median |h error| 0.037, 6.8
+    fixed-point iterations per solve; 0.2 -- 0.023, 8.3; 0.4 -- 0.18, 11.0.  0.1 is the
+    largest size at which the solves stay below 7 iterations."""
+    rng = np.random.default_rng(seed)
+    g = rng.standard_normal((dim, dim))
+    prec = np.identity(dim) + 0.1 * (g @ g.T) / dim
+    base = np.linalg.cholesky(prec)
+    coeff = 1.0 / dim if coeff is None else float(coeff)
+    pos = 0.5 * rng.standard_normal((n_chains, dim))
+    z = rng.standard_normal((n_chains, dim))
+    # L(q) z = L0 z + c q o cumsum(q o z): the rows of tril(q q^T) z
+    mom = z @ base.T + coeff * pos * np.cumsum(pos * z, axis=1)
+    return Problem(
+        name="C8",
+        integrator=integrator,
+        system="cholesky_riemannian",
+        target="quadratic",
+        target_params={"prec": prec},
+        step_size=step_size,
+        pos=pos,
+        mom=mom,
+        metric_model="chol_quadratic",
+        metric_params={"base_factor": base, "coeff": coeff},
+    )
+
+
 def sphere_constrained(n_chains=64, dim=10, seed=BASE_SEED + 5, metric_kind="dense",
                        dens_wrt_hausdorff=True):
     """Extra parity case for K6 beyond C3: unit sphere in R^dim, tilted Gaussian density,
@@ -393,6 +432,7 @@ CONFIGS = {
     "C5": c5_dense_hadamard,
     "C6": c6_softabs_quartic,
     "C7": c7_funnel_riemannian,
+    "C8": c8_cholesky_riemannian,
     "S1": sphere_constrained,
     "S2": multi_sphere_constrained,
     "G1": g1_gaussian_split,

@@ -8,6 +8,7 @@ hot path:
 * ``SoftAbsRiemannianMetricSystem``           systems.py:1763-1920
 * ``ScalarRiemannianMetricSystem``            systems.py:1405-1490
 * ``DiagonalRiemannianMetricSystem``          systems.py:1493-1571
+* ``CholeskyFactoredRiemannianMetricSystem``  systems.py:1574-1653
 
 Differences forced by the device: ``neg_log_dens`` is an instance of
 ``mici_b200.targets.Target`` (a model compiled into the library) instead of a Python callable,
@@ -30,6 +31,7 @@ from .targets import (
     FunnelFisherMetric,
     HadamardMetric,
     NealFunnel,
+    QuadraticCholeskyMetric,
     QuadraticDiagonalMetric,
     QuadraticScalarMetric,
     Rank1Metric,
@@ -671,3 +673,34 @@ class DiagonalRiemannianMetricSystem(RiemannianMetricSystem):
         self.metric_model = metric_diagonal_func
         self._rmetric_id = metric_diagonal_func.rmetric_id
         self._rmetric_params = metric_diagonal_func.params
+
+
+class CholeskyFactoredRiemannianMetricSystem(RiemannianMetricSystem):
+    """Position-dependent metric given by its lower-triangular Cholesky factor,
+    ``M(q) = L(q) L(q)^T`` (systems.py:1574-1653), with ``TriangularFactoredPositiveDefiniteMatrix``
+    arithmetic (matrices.py:795-1114): ``metric_chol_func`` is a registered metric model,
+    ``mici_b200.targets.QuadraticCholeskyMetric`` (L = L0 + c tril(q q^T)).  No factorisation:
+    each metric evaluation fills L and solves with it, O(D^2) per chain, with L in shared memory
+    up to D of about 150 and in a per-CTA global workspace beyond.
+
+    Failures follow the reference's matrix class: a non-finite entry of L fails when the metric
+    is built -- status 3 (``LinAlgError``) outside a fixed-point solve, ``ConvergenceError``
+    inside one.  A negative diagonal entry is legal.  A zero diagonal entry fails only where the
+    metric is solved with: ``dh_dmom`` raises ``LinAlgError``, ``h`` is NaN, ``sample_momentum``
+    succeeds, and an integrator step ends in ``ConvergenceError`` (DESIGN.md section 1)."""
+
+    def __init__(self, neg_log_dens, metric_chol_func, *, vjp_metric_chol_func=None,
+                 grad_neg_log_dens=None, backend=None):
+        super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
+        if not isinstance(metric_chol_func, QuadraticCholeskyMetric):
+            raise TypeError("`metric_chol_func` must be a registered metric model "
+                            "(QuadraticCholeskyMetric).")
+        if vjp_metric_chol_func is not None:
+            raise ValueError("The metric VJP is fused into the kernels.")
+        if metric_chol_func.dim != neg_log_dens.dim:
+            raise ValueError(f"The base factor is {metric_chol_func.dim} x {metric_chol_func.dim}; "
+                             f"the target has dimension {neg_log_dens.dim}.")
+        self.metric_model = metric_chol_func
+        self._rmetric_id = metric_chol_func.rmetric_id
+        self._rmetric_params = metric_chol_func.params
+        self._rmetric_aux = metric_chol_func.aux

@@ -26,6 +26,7 @@ RMETRIC_HADAMARD = 2
 RMETRIC_DIAG_QUADRATIC = 3
 RMETRIC_DIAG_FUNNEL_FISHER = 4
 RMETRIC_SCALAR_QUADRATIC = 5
+RMETRIC_CHOL_QUADRATIC = 6
 
 
 class Target:
@@ -229,6 +230,35 @@ class QuadraticScalarMetric:
         self.params = (a, b)
 
 
+class QuadraticCholeskyMetric:
+    """Position-dependent metric M(q) = L(q) L(q)^T given by its lower-triangular factor
+    L(q) = L0 + c tril(q q^T) (``CholeskyFactoredRiemannianMetricSystem``).  Only the lower
+    triangle of ``base_factor`` is used: its upper triangle is zeroed, as the reference does for
+    every factor it is given.
+
+    M(q) is positive definite wherever every diagonal entry L_ii(q) = (L0)_ii + c q_i^2 is
+    non-zero; ``coeff >= 0`` with a positive diagonal of ``L0`` guarantees that at every finite
+    q.  Any finite square ``L0`` and finite ``coeff`` are accepted, so that factors with
+    negative or vanishing diagonal entries behave as in the reference: a negative entry is
+    legal (only |L_ii| enters log|M|), a zero one fails wherever the metric is solved with."""
+
+    rmetric_id = RMETRIC_CHOL_QUADRATIC
+    name = "chol_quadratic"
+
+    def __init__(self, base_factor, coeff):
+        base = np.asarray(base_factor, dtype=np.float64)
+        coeff = float(coeff)
+        if base.ndim != 2 or base.shape[0] != base.shape[1]:
+            raise ValueError("`base_factor` must be a square matrix.")
+        if not np.all(np.isfinite(base)) or not np.isfinite(coeff):
+            raise ValueError("`base_factor` and `coeff` must be finite.")
+        self.base_factor = np.ascontiguousarray(np.tril(base))
+        self.coeff = coeff
+        self.dim = base.shape[0]
+        self.aux = self.base_factor
+        self.params = (coeff,)
+
+
 REGISTRY = {
     cls.name: cls
     for cls in (StdGaussian, NealFunnel, Banana, Quadratic, Quartic, Torus, Sphere, MultiSphere)
@@ -236,7 +266,7 @@ REGISTRY = {
 METRIC_REGISTRY = {
     cls.name: cls
     for cls in (Rank1Metric, HadamardMetric, QuadraticDiagonalMetric, FunnelFisherMetric,
-                QuadraticScalarMetric)
+                QuadraticScalarMetric, QuadraticCholeskyMetric)
 }
 
 
