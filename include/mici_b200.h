@@ -208,6 +208,30 @@ int mb200_constrained_leapfrog_euclidean(
     int32_t* n_done, int32_t* newton_iters, void* stream);
 
 /*
+ * The same for GaussianDenseConstrainedEuclideanMetricSystem (systems.py:1034-1184): h2 =
+ * q.q/2 + p.M^-1 p/2, whose flow is the exact rotation of (q, p) in the eigenbasis of M; the
+ * projection solvers use dh2_flow_dmom(|dt|) = (U diag(sin(w|dt|) w) U^T, U diag(cos(w|dt|)) U^T);
+ * the Gram matrices are inverted through their eigendecomposition (DenseSymmetricMatrix); the
+ * density is always with respect to the Lebesgue measure.  With (eigval, U) the metric's
+ * eigendecomposition:
+ *   metric_omega    [dim] w = 1 / eigval^(1/2) (device; ones for the identity metric)
+ *   metric_eigvec   [dim*dim] U, row-major (device; dense metric only, else NULL)
+ *   metric_eigvec_t [dim*dim] U^T, row-major (device; dense metric only, else NULL)
+ * sin(w |dt|) and cos(w |dt|) are evaluated per chain, so step_sizes may vary per chain with
+ * every metric kind.  Other arguments, targets and sizes as for
+ * mb200_constrained_leapfrog_euclidean.
+ */
+int mb200_constrained_leapfrog_gaussian_euclidean(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const double* metric_omega, const double* metric_eigvec,
+    const double* metric_eigvec_t, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream);
+
+/*
  * n_steps implicit generalised-leapfrog steps on a Riemannian-metric system, fixed-point
  * solves by direct iteration.
  * Replaces: ImplicitLeapfrogIntegrator.step (integrators.py:482-544; NB every sub-map gets the
@@ -319,6 +343,12 @@ int mb200_project_onto_cotangent_space(const double* pos, const double* mom_in, 
                                        int64_t n_chains, int32_t dim, int32_t metric_kind,
                                        const double* metric_inv, const mb200_model* model,
                                        void* stream);
+/* The same projection with the Gram matrix inverted through its eigendecomposition, as
+ * GaussianDenseConstrainedEuclideanMetricSystem does (systems.py:1157-1169). */
+int mb200_project_onto_cotangent_space_gaussian(const double* pos, const double* mom_in,
+                                                double* mom_out, int64_t n_chains, int32_t dim,
+                                                int32_t metric_kind, const double* metric_inv,
+                                                const mb200_model* model, void* stream);
 int mb200_sample_momentum_riemannian(const double* pos, const double* normals, double* mom_out,
                                      int64_t n_chains, int32_t dim, const mb200_model* model,
                                      int32_t* status, void* stream);

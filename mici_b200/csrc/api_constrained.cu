@@ -5,39 +5,170 @@
 
 namespace mb200 {
 
-template <class Target, int KP>
+// The Gaussian split's w vector and eigenvector matrices (all NULL for the plain system)
+struct GaussianArgs {
+  const double* omega;
+  const double* eigvec;
+  const double* eigvec_t;
+};
+
+template <bool GAUSS, class Target, int KP>
 static int launch_constrained(const double* q_in, const double* p_in, double* q_out,
                               double* p_out, const int32_t* dir, int64_t n, int dim, double eps,
                               int n_steps, int n_inner, int metric_kind, const double* minv,
                               const ModelArgs& m, double ctol, double ptol, double dtol,
                               int max_iters, double rev_tol, double* h_out, int32_t* status,
                               int32_t* n_done, int32_t* iters, cudaStream_t st, int proj_solver,
-                              int max_ls) {
+                              int max_ls, const GaussianArgs& ga) {
   constexpr int WARPS = 4;
-  auto kern = constrained_leapfrog_kernel<Target, KP>;
-  const size_t smem = (size_t)WARPS * (Target::NC > 1 ? Target::NC : 1) * 64 * KP * sizeof(double);
+  auto kern = constrained_leapfrog_kernel<Target, KP, GAUSS>;
+  const size_t smem =
+      (size_t)WARPS * constrained_smem_per_warp<Target::NC, KP, GAUSS>() * sizeof(double);
   int64_t blocks = (n + WARPS - 1) / WARPS;
   const int64_t cap = (int64_t)num_sms() * 16;
   if (blocks > cap) blocks = cap;
   kern<<<(unsigned)blocks, WARPS * 32, smem, st>>>(q_in, p_in, q_out, p_out, dir, n, dim, eps,
                                                    n_steps, n_inner, metric_kind, minv, m, ctol,
                                                    ptol, dtol, max_iters, rev_tol, h_out, status,
-                                                   n_done, iters, proj_solver, max_ls);
+                                                   n_done, iters, proj_solver, max_ls, ga.omega,
+                                                   ga.eigvec, ga.eigvec_t);
   return check_launch("constrained_leapfrog_kernel");
 }
 
-template <class Target, int KP>
+template <bool GAUSS, class Target, int KP>
 static int launch_project(const double* q, const double* p_in, double* p_out, int64_t n, int dim,
                           int metric_kind, const double* minv, const ModelArgs& m,
                           cudaStream_t st) {
   constexpr int WARPS = 4;
-  const size_t smem = (size_t)WARPS * (Target::NC > 1 ? Target::NC : 1) * 64 * KP * sizeof(double);
+  const size_t smem =
+      (size_t)WARPS * constrained_smem_per_warp<Target::NC, KP, GAUSS>() * sizeof(double);
   int64_t blocks = (n + WARPS - 1) / WARPS;
   const int64_t cap = (int64_t)num_sms() * 16;
   if (blocks > cap) blocks = cap;
-  constrained_project_kernel<Target, KP><<<(unsigned)blocks, WARPS * 32, smem, st>>>(
+  constrained_project_kernel<Target, KP, GAUSS><<<(unsigned)blocks, WARPS * 32, smem, st>>>(
       q, p_in, p_out, n, dim, metric_kind, minv, m);
   return check_launch("constrained_project_kernel");
+}
+
+// Argument checks and target / size dispatch shared by the plain and the Gaussian-split entry
+// points (the torus one-thread kernel serves the plain system's Hausdorff density only).
+template <bool GAUSS>
+static int constrained_leapfrog_dispatch(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const GaussianArgs& ga, const mb200_model* model,
+    int32_t projection_solver, double constraint_tol, double position_tol, double divergence_tol,
+    int32_t max_iters, int32_t max_line_search_iters, double reverse_check_tol, double* h_out,
+    int32_t* status, int32_t* n_done, int32_t* newton_iters, void* stream) {
+  if (n_chains == 0 && dim >= 1) return 0;
+  if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
+    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_chains < 0 || dim < 1 || n_steps < 0 || n_inner_step < 1 || max_iters < 0 ||
+      max_line_search_iters < 0)
+    return fail(MB200_ERR_INVALID_ARG, "bad sizes");
+  if (projection_solver < 0 || projection_solver > 2)
+    return fail(MB200_ERR_INVALID_ARG, "unknown projection solver %d", projection_solver);
+  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
+  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
+    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
+  if (GAUSS && !ga.omega) return fail(MB200_ERR_INVALID_ARG, "metric_omega is NULL");
+  if (GAUSS && metric_kind == MB200_METRIC_DENSE && (!ga.eigvec || !ga.eigvec_t))
+    return fail(MB200_ERR_INVALID_ARG, "metric_eigvec / metric_eigvec_t is NULL");
+  if (n_chains == 0) return 0;
+  const DeviceScope device_scope(pos_in);
+  const ModelArgs m = to_args(model, step_sizes, n_steps_per_chain);
+  cudaStream_t st = (cudaStream_t)stream;
+#define MB200_ARGS                                                                              \
+  pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps, n_inner_step,       \
+      metric_kind, metric_inv, m, constraint_tol, position_tol, divergence_tol, max_iters,      \
+      reverse_check_tol, h_out, status, n_done, newton_iters, st, projection_solver,            \
+      max_line_search_iters, ga
+  switch (m.target_id) {
+    case MB200_TARGET_TORUS:
+      if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
+      // config C3: identity metric, Newton projection, Hausdorff density -> one THREAD per chain
+      if (!GAUSS && metric_kind == MB200_METRIC_IDENTITY &&
+          projection_solver == MB200_PROJ_SOLVER_NEWTON && m.tp[MB200_MAX_PARAMS - 1] == 0.0) {
+        // latency bound per chain: spread small batches over as many warps as there are
+        // sub-partitions (measured: 8 lanes per warp 0.287 ms, 32 lanes 0.300 ms at 4096 chains)
+        const int lanes = n_chains >= (int64_t)num_sms() * 4 * 32 ? 32 : 8;
+        int64_t blocks = (n_chains + lanes - 1) / lanes;
+        const int64_t cap = (int64_t)num_sms() * 16;
+        if (blocks > cap) blocks = cap;
+        constrained_torus_thread_kernel<<<(unsigned)blocks, 32, 0, st>>>(
+            pos_in, mom_in, pos_out, mom_out, dir, n_chains, step_size, n_steps, n_inner_step, m,
+            constraint_tol, position_tol, divergence_tol, max_iters, reverse_check_tol, h_out,
+            status, n_done, newton_iters, lanes);
+        return check_launch("constrained_torus_thread_kernel");
+      }
+      return launch_constrained<GAUSS, TorusTarget, 1>(MB200_ARGS);
+    case MB200_TARGET_SPHERE:
+      if (dim <= 64) return launch_constrained<GAUSS, SphereTarget, 1>(MB200_ARGS);
+      if (dim <= 128) return launch_constrained<GAUSS, SphereTarget, 2>(MB200_ARGS);
+      if (dim <= 256) return launch_constrained<GAUSS, SphereTarget, 4>(MB200_ARGS);
+      return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
+    case MB200_TARGET_MULTI_SPHERE: {
+      const int nc = (int)m.tp[0];
+      if ((nc != 2 && nc != 4 && nc != 8) || dim % nc != 0 || dim > 128)
+        return fail(MB200_ERR_UNSUPPORTED,
+                    "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
+      if (dim <= 64) {
+        if (nc == 2) return launch_constrained<GAUSS, MultiSphereTarget<2>, 1>(MB200_ARGS);
+        if (nc == 4) return launch_constrained<GAUSS, MultiSphereTarget<4>, 1>(MB200_ARGS);
+        return launch_constrained<GAUSS, MultiSphereTarget<8>, 1>(MB200_ARGS);
+      }
+      if (nc == 2) return launch_constrained<GAUSS, MultiSphereTarget<2>, 2>(MB200_ARGS);
+      if (nc == 4) return launch_constrained<GAUSS, MultiSphereTarget<4>, 2>(MB200_ARGS);
+      return launch_constrained<GAUSS, MultiSphereTarget<8>, 2>(MB200_ARGS);
+    }
+    default:
+      return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
+  }
+#undef MB200_ARGS
+}
+
+template <bool GAUSS>
+static int project_dispatch(const double* pos, const double* mom_in, double* mom_out,
+                            int64_t n_chains, int32_t dim, int32_t metric_kind,
+                            const double* metric_inv, const mb200_model* model, void* stream) {
+  if (n_chains == 0 && dim >= 1) return 0;
+  if (!pos || !mom_in || !mom_out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
+  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
+  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
+    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
+  const DeviceScope device_scope(pos);
+  const ModelArgs m = to_args(model);
+  cudaStream_t st = (cudaStream_t)stream;
+#define MB200_ARGS pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv, m, st
+  switch (m.target_id) {
+    case MB200_TARGET_TORUS:
+      if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
+      return launch_project<GAUSS, TorusTarget, 1>(MB200_ARGS);
+    case MB200_TARGET_SPHERE:
+      if (dim <= 64) return launch_project<GAUSS, SphereTarget, 1>(MB200_ARGS);
+      if (dim <= 128) return launch_project<GAUSS, SphereTarget, 2>(MB200_ARGS);
+      if (dim <= 256) return launch_project<GAUSS, SphereTarget, 4>(MB200_ARGS);
+      return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
+    case MB200_TARGET_MULTI_SPHERE: {
+      const int nc = (int)m.tp[0];
+      if ((nc != 2 && nc != 4 && nc != 8) || dim % nc != 0 || dim > 128)
+        return fail(MB200_ERR_UNSUPPORTED,
+                    "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
+      if (dim <= 64) {
+        if (nc == 2) return launch_project<GAUSS, MultiSphereTarget<2>, 1>(MB200_ARGS);
+        if (nc == 4) return launch_project<GAUSS, MultiSphereTarget<4>, 1>(MB200_ARGS);
+        return launch_project<GAUSS, MultiSphereTarget<8>, 1>(MB200_ARGS);
+      }
+      if (nc == 2) return launch_project<GAUSS, MultiSphereTarget<2>, 2>(MB200_ARGS);
+      if (nc == 4) return launch_project<GAUSS, MultiSphereTarget<4>, 2>(MB200_ARGS);
+      return launch_project<GAUSS, MultiSphereTarget<8>, 2>(MB200_ARGS);
+    }
+    default:
+      return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
+  }
+#undef MB200_ARGS
 }
 
 }  // namespace mb200
@@ -54,111 +185,44 @@ int mb200_constrained_leapfrog_euclidean(
     double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
     int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
     int32_t* n_done, int32_t* newton_iters, void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
-    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1 || n_steps < 0 || n_inner_step < 1 || max_iters < 0 ||
-      max_line_search_iters < 0)
-    return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  if (projection_solver < 0 || projection_solver > 2)
-    return fail(MB200_ERR_INVALID_ARG, "unknown projection solver %d", projection_solver);
-  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
-  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
-    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
-  if (n_chains == 0) return 0;
-  const DeviceScope device_scope(pos_in);
-  const ModelArgs m = to_args(model, step_sizes, n_steps_per_chain);
-  cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS                                                                              \
-  pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps, n_inner_step,       \
-      metric_kind, metric_inv, m, constraint_tol, position_tol, divergence_tol, max_iters,      \
-      reverse_check_tol, h_out, status, n_done, newton_iters, st, projection_solver,            \
-      max_line_search_iters
-  switch (m.target_id) {
-    case MB200_TARGET_TORUS:
-      if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
-      // config C3: identity metric, Newton projection, Hausdorff density -> one THREAD per chain
-      if (metric_kind == MB200_METRIC_IDENTITY && projection_solver == MB200_PROJ_SOLVER_NEWTON &&
-          m.tp[MB200_MAX_PARAMS - 1] == 0.0) {
-        // latency bound per chain: spread small batches over as many warps as there are
-        // sub-partitions (measured: 8 lanes per warp 0.287 ms, 32 lanes 0.300 ms at 4096 chains)
-        const int lanes = n_chains >= (int64_t)num_sms() * 4 * 32 ? 32 : 8;
-        int64_t blocks = (n_chains + lanes - 1) / lanes;
-        const int64_t cap = (int64_t)num_sms() * 16;
-        if (blocks > cap) blocks = cap;
-        constrained_torus_thread_kernel<<<(unsigned)blocks, 32, 0, st>>>(
-            pos_in, mom_in, pos_out, mom_out, dir, n_chains, step_size, n_steps, n_inner_step, m,
-            constraint_tol, position_tol, divergence_tol, max_iters, reverse_check_tol, h_out,
-            status, n_done, newton_iters, lanes);
-        return check_launch("constrained_torus_thread_kernel");
-      }
-      return launch_constrained<TorusTarget, 1>(MB200_ARGS);
-    case MB200_TARGET_SPHERE:
-      if (dim <= 64) return launch_constrained<SphereTarget, 1>(MB200_ARGS);
-      if (dim <= 128) return launch_constrained<SphereTarget, 2>(MB200_ARGS);
-      if (dim <= 256) return launch_constrained<SphereTarget, 4>(MB200_ARGS);
-      return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
-    case MB200_TARGET_MULTI_SPHERE: {
-      const int nc = (int)m.tp[0];
-      if ((nc != 2 && nc != 4 && nc != 8) || dim % nc != 0 || dim > 128)
-        return fail(MB200_ERR_UNSUPPORTED,
-                    "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
-      if (dim <= 64) {
-        if (nc == 2) return launch_constrained<MultiSphereTarget<2>, 1>(MB200_ARGS);
-        if (nc == 4) return launch_constrained<MultiSphereTarget<4>, 1>(MB200_ARGS);
-        return launch_constrained<MultiSphereTarget<8>, 1>(MB200_ARGS);
-      }
-      if (nc == 2) return launch_constrained<MultiSphereTarget<2>, 2>(MB200_ARGS);
-      if (nc == 4) return launch_constrained<MultiSphereTarget<4>, 2>(MB200_ARGS);
-      return launch_constrained<MultiSphereTarget<8>, 2>(MB200_ARGS);
-    }
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
-  }
-#undef MB200_ARGS
+  return constrained_leapfrog_dispatch<false>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, n_inner_step, metric_kind, metric_inv, GaussianArgs{nullptr, nullptr, nullptr},
+      model, projection_solver, constraint_tol, position_tol, divergence_tol, max_iters,
+      max_line_search_iters, reverse_check_tol, h_out, status, n_done, newton_iters, stream);
+}
+
+int mb200_constrained_leapfrog_gaussian_euclidean(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const double* metric_omega, const double* metric_eigvec,
+    const double* metric_eigvec_t, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream) {
+  return constrained_leapfrog_dispatch<true>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, n_inner_step, metric_kind, metric_inv,
+      GaussianArgs{metric_omega, metric_eigvec, metric_eigvec_t}, model, projection_solver,
+      constraint_tol, position_tol, divergence_tol, max_iters, max_line_search_iters,
+      reverse_check_tol, h_out, status, n_done, newton_iters, stream);
 }
 
 int mb200_project_onto_cotangent_space(const double* pos, const double* mom_in, double* mom_out,
                                        int64_t n_chains, int32_t dim, int32_t metric_kind,
                                        const double* metric_inv, const mb200_model* model,
                                        void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos || !mom_in || !mom_out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
-  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
-    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
-  const DeviceScope device_scope(pos);
-  const ModelArgs m = to_args(model);
-  cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv, m, st
-  switch (m.target_id) {
-    case MB200_TARGET_TORUS:
-      if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
-      return launch_project<TorusTarget, 1>(MB200_ARGS);
-    case MB200_TARGET_SPHERE:
-      if (dim <= 64) return launch_project<SphereTarget, 1>(MB200_ARGS);
-      if (dim <= 128) return launch_project<SphereTarget, 2>(MB200_ARGS);
-      if (dim <= 256) return launch_project<SphereTarget, 4>(MB200_ARGS);
-      return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
-    case MB200_TARGET_MULTI_SPHERE: {
-      const int nc = (int)m.tp[0];
-      if ((nc != 2 && nc != 4 && nc != 8) || dim % nc != 0 || dim > 128)
-        return fail(MB200_ERR_UNSUPPORTED,
-                    "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
-      if (dim <= 64) {
-        if (nc == 2) return launch_project<MultiSphereTarget<2>, 1>(MB200_ARGS);
-        if (nc == 4) return launch_project<MultiSphereTarget<4>, 1>(MB200_ARGS);
-        return launch_project<MultiSphereTarget<8>, 1>(MB200_ARGS);
-      }
-      if (nc == 2) return launch_project<MultiSphereTarget<2>, 2>(MB200_ARGS);
-      if (nc == 4) return launch_project<MultiSphereTarget<4>, 2>(MB200_ARGS);
-      return launch_project<MultiSphereTarget<8>, 2>(MB200_ARGS);
-    }
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
-  }
-#undef MB200_ARGS
+  return project_dispatch<false>(pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv,
+                                 model, stream);
+}
+
+int mb200_project_onto_cotangent_space_gaussian(const double* pos, const double* mom_in,
+                                                double* mom_out, int64_t n_chains, int32_t dim,
+                                                int32_t metric_kind, const double* metric_inv,
+                                                const mb200_model* model, void* stream) {
+  return project_dispatch<true>(pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv,
+                                model, stream);
 }
 
 }  // extern "C"

@@ -11,7 +11,8 @@
 // metric_ops.cuh.  Every branch (Newton convergence, divergence, reversibility failure) is
 // uniform across the warp, so chains in other warps proceed independently: the per-chain
 // convergence mask of the reference's Python loop is the warp's own control flow.  The C x C
-// systems (C = Target::NC <= 4) are solved redundantly in registers by every lane.
+// systems (C = Target::NC <= 8) are solved redundantly in registers by every lane.  The same
+// kernels with GAUSS = true run GaussianDenseConstrainedEuclideanMetricSystem (systems.py:1034-1184).
 #pragma once
 #include "metric_ops.cuh"
 #include "targets.cuh"
@@ -368,7 +369,95 @@ __device__ __forceinline__ void lu_solve(double (&R)[C][C], const double (&c)[C]
   }
 }
 
-template <class Target, int KP>
+// Eigendecomposition G = V diag(lam) V^T of a symmetric C x C matrix by cyclic Jacobi rotations
+// (every lane redundantly, only the upper triangle of A is read and written).  Stands in for
+// numpy.linalg.eigh of DenseSymmetricMatrix (matrices.py:436-438); at C = 1 it returns lam = G,
+// V = 1 exactly as LAPACK does.  The eigenvalues come out unsorted; a non-finite entry makes
+// every output NaN-contaminated, which the callers' NaN tests turn into a ConvergenceError.
+template <int C>
+__device__ __forceinline__ void jacobi_eigh(const double (&G)[C][C], double (&lam)[C],
+                                            double (&V)[C][C]) {
+  double A[C][C];
+#pragma unroll
+  for (int i = 0; i < C; ++i)
+#pragma unroll
+    for (int j = 0; j < C; ++j) A[i][j] = G[i][j], V[i][j] = (i == j) ? 1.0 : 0.0;
+#pragma unroll 1
+  for (int sweep = 0; sweep < 16; ++sweep) {
+    double off = 0.0;
+#pragma unroll
+    for (int i = 0; i < C; ++i)
+#pragma unroll
+      for (int j = i + 1; j < C; ++j) off = fma(A[i][j], A[i][j], off);
+    if (!(off > 0.0)) break;  // diagonal, or NaN
+#pragma unroll
+    for (int p = 0; p < C; ++p)
+#pragma unroll
+      for (int q = p + 1; q < C; ++q) {
+        const double apq = A[p][q];
+        const double g = 100.0 * fabs(apq);
+        if (sweep > 3 && fabs(A[p][p]) + g == fabs(A[p][p]) && fabs(A[q][q]) + g == fabs(A[q][q])) {
+          A[p][q] = 0.0;  // below the diagonal's resolution (Numerical Recipes' jacobi)
+        } else if (apq != 0.0) {
+          const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
+          const double tn = copysign(1.0, theta) / (fabs(theta) + sqrt(fma(theta, theta, 1.0)));
+          const double c = 1.0 / sqrt(fma(tn, tn, 1.0)), s = tn * c;
+          A[p][p] -= tn * apq;
+          A[q][q] += tn * apq;
+          A[p][q] = 0.0;
+#pragma unroll
+          for (int r = 0; r < C; ++r) {
+            if (r == p || r == q) continue;
+            double& arp = r < p ? A[r][p] : A[p][r];
+            double& arq = r < q ? A[r][q] : A[q][r];
+            const double x = arp, y = arq;
+            arp = c * x - s * y;
+            arq = s * x + c * y;
+          }
+#pragma unroll
+          for (int r = 0; r < C; ++r) {
+            const double x = V[r][p], y = V[r][q];
+            V[r][p] = c * x - s * y;
+            V[r][q] = s * x + c * y;
+          }
+        }
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < C; ++i) lam[i] = A[i][i];
+}
+
+// x = G^-1 u with G^-1 = EigendecomposedSymmetricMatrix(V, 1 / lam), the inverse of a
+// DenseSymmetricMatrix (matrices.py:1446-1447, 1568-1569): V (diag(1/lam) (V^T u)).
+template <int C>
+__device__ __forceinline__ void eig_inverse_apply(const double (&lam)[C], const double (&V)[C][C],
+                                                  const double (&u)[C], double (&x)[C]) {
+  double y[C];
+#pragma unroll
+  for (int i = 0; i < C; ++i) {
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < C; ++k) s = fma(V[k][i], u[k], s);
+    y[i] = (1.0 / lam[i]) * s;
+  }
+#pragma unroll
+  for (int i = 0; i < C; ++i) {
+    double s = 0.0;
+#pragma unroll
+    for (int k = 0; k < C; ++k) s = fma(V[i][k], y[k], s);
+    x[i] = s;
+  }
+}
+
+// Per-chain data of the Gaussian split (GaussianEuclideanMetricSystem, systems.py:464-474, and
+// dh2_flow_dmom, systems.py:1171-1184): w = 1 / eigval^(1/2) of the metric and sin(w |dt|),
+// cos(w |dt|) for the chain's inner step, in the pair layout of the eigen-coordinates.
+template <int NV>
+struct GaussianRotation {
+  double om[NV], sw[NV], cw[NV];
+};
+
+template <class Target, int KP, bool GAUSS = false>
 struct ConstrainedOps {
   static constexpr int NV = 2 * KP;
   static constexpr int C = Target::NC;
@@ -379,6 +468,141 @@ struct ConstrainedOps {
   int dim, lane;
   double* psm;
   int solver, max_ls;
+  // GAUSS only: w and the metric's eigenvectors U (row-major) and U^T (NULL unless dense)
+  const double* omega = nullptr;
+  const double* eigvec = nullptr;
+  const double* eigvec_t = nullptr;
+  GaussianRotation<NV> rot = {};
+
+  // sin / cos of w |dt| for this chain (CUDA's sincos; NumPy's sin / cos may differ in the last
+  // bit).  Padding coordinates get w = 1 and hold zeros.
+  __device__ __forceinline__ void set_rotation(double adt) {
+#pragma unroll
+    for (int e = 0; e < NV; ++e) {
+      const int i = 2 * lane + 64 * (e >> 1) + (e & 1);
+      const double om = (i < dim) ? omega[i] : 1.0;
+      rot.om[e] = om;
+      sincos(om * adt, &rot.sw[e], &rot.cw[e]);
+    }
+  }
+  // R vectors to eigen-coordinates, U^T x (inv_metric_apply forms A^T x, A = U), and back, U y
+  // (A = U^T).  Identity and diagonal metrics have U = I and skip the products.
+  template <int R>
+  __device__ __forceinline__ void to_eig(const double (&a)[R][NV], double (&out)[R][NV]) const {
+    inv_metric_apply<KP, R>(metric_kind == MB200_METRIC_DENSE ? MB200_METRIC_DENSE
+                                                              : MB200_METRIC_IDENTITY,
+                            eigvec, dim, lane, psm, a, out);
+  }
+  template <int R>
+  __device__ __forceinline__ void from_eig(const double (&a)[R][NV], double (&out)[R][NV]) const {
+    inv_metric_apply<KP, R>(metric_kind == MB200_METRIC_DENSE ? MB200_METRIC_DENSE
+                                                              : MB200_METRIC_IDENTITY,
+                            eigvec_t, dim, lane, psm, a, out);
+  }
+
+  // h2_flow(dt): q += dt M^-1 p (systems.py:362-363), or for the Gaussian split the exact
+  // rotation (systems.py:464-474), rotated in the eigenbasis, then multiplied and added:
+  //   q' = U (cos(w dt) U^T q + (sin(w dt) w) U^T p),  p' = U (cos(w dt) U^T p - (sin(w dt)/w) U^T q)
+  __device__ __forceinline__ void drift(double (&q)[NV], double (&p)[NV], double dt) const {
+    if constexpr (GAUSS) {
+      double x[2][NV], y[2][NV];
+#pragma unroll
+      for (int e = 0; e < NV; ++e) x[0][e] = q[e], x[1][e] = p[e];
+      to_eig<2>(x, y);
+      const double sgn = dt < 0.0 ? -1.0 : 1.0;  // sin is odd: sin(w dt) = sgn sin(w |dt|)
+#pragma unroll
+      for (int e = 0; e < NV; ++e) {
+        const double sn = sgn * rot.sw[e], cs = rot.cw[e], om = rot.om[e];
+        x[0][e] = __dadd_rn(__dmul_rn(cs, y[0][e]), __dmul_rn(__dmul_rn(sn, om), y[1][e]));
+        x[1][e] = __dsub_rn(__dmul_rn(cs, y[1][e]), __dmul_rn(__ddiv_rn(sn, om), y[0][e]));
+      }
+      from_eig<2>(x, y);
+#pragma unroll
+      for (int e = 0; e < NV; ++e) q[e] = y[0][e], p[e] = y[1][e];
+    } else {
+      double v[NV];
+      inv_metric_vec(p, v);
+#pragma unroll
+      for (int e = 0; e < NV; ++e) q[e] = __dadd_rn(q[e], __dmul_rn(dt, v[e]));
+    }
+  }
+
+  // S_a = dh2_flow_pos_dmom(|dt|) Jp_a^T: |dt| M^-1 Jp_a^T (systems.py:794-799), or
+  // U (sin(w |dt|) w  .*  U^T Jp_a^T) for the Gaussian split (systems.py:1171-1184)
+  __device__ __forceinline__ void flow_rows(const double (&Jp)[C][NV], double adt,
+                                            double (&S)[C][NV]) const {
+    if constexpr (GAUSS) {
+      double y[C][NV];
+      to_eig<C>(Jp, y);
+#pragma unroll
+      for (int a = 0; a < C; ++a)
+#pragma unroll
+        for (int e = 0; e < NV; ++e) y[a][e] = __dmul_rn(__dmul_rn(rot.sw[e], rot.om[e]), y[a][e]);
+      from_eig<C>(y, S);
+    } else {
+      inv_metric_rows(Jp, S);
+#pragma unroll
+      for (int a = 0; a < C; ++a)
+#pragma unroll
+        for (int e = 0; e < NV; ++e) S[a][e] = adt * S[a][e];
+    }
+  }
+
+  // on convergence: p -= sign(dt) dh2_flow_mom_dmom mu (solvers.py:331, 457, 586), with
+  // dh2_flow_mom_dmom = I, or U diag(cos(w |dt|)) U^T for the Gaussian split
+  __device__ __forceinline__ void finish(double (&p)[NV], const double (&mu)[NV], double dt) const {
+    const double sgn = (dt > 0.0) ? 1.0 : ((dt < 0.0) ? -1.0 : 0.0);
+    if constexpr (GAUSS) {
+      double x[1][NV], y[1][NV];
+#pragma unroll
+      for (int e = 0; e < NV; ++e) x[0][e] = mu[e];
+      to_eig<1>(x, y);
+#pragma unroll
+      for (int e = 0; e < NV; ++e) y[0][e] = __dmul_rn(sgn * rot.cw[e], y[0][e]);
+      from_eig<1>(y, x);
+#pragma unroll
+      for (int e = 0; e < NV; ++e) p[e] = __dsub_rn(p[e], x[0][e]);
+    } else {
+#pragma unroll
+      for (int e = 0; e < NV; ++e) p[e] = __dsub_rn(p[e], sgn * mu[e]);
+    }
+  }
+
+  // Gram-matrix inverse: DensePositiveDefiniteMatrix (Cholesky) for DenseConstrained...System
+  // (systems.py:1006-1022), DenseSymmetricMatrix (eigh) for the Gaussian one (:1157-1169)
+  __device__ __forceinline__ void gram_solve(const double (&G)[C][C], const double (&u)[C],
+                                             double (&x)[C]) const {
+    if constexpr (GAUSS) {
+      double lam[C], V[C][C];
+      jacobi_eigh<C>(G, lam, V);
+      eig_inverse_apply<C>(lam, V, u, x);
+    } else {
+      spd_inverse_apply<C>(G, u, x);
+    }
+  }
+  __device__ __forceinline__ void gram_inverse_logdet(const double (&G)[C][C],
+                                                      double (&Ginv)[C][C],
+                                                      double& half_logdet) const {
+    if constexpr (GAUSS) {
+      double lam[C], V[C][C];
+      jacobi_eigh<C>(G, lam, V);
+      double s = 0.0;  // SymmetricMatrix.log_abs_det (matrices.py:457-459)
+#pragma unroll
+      for (int i = 0; i < C; ++i) s += log(fabs(lam[i]));
+      half_logdet = 0.5 * s;
+#pragma unroll
+      for (int a = 0; a < C; ++a)
+#pragma unroll
+        for (int b = 0; b < C; ++b) {
+          double v = 0.0;
+#pragma unroll
+          for (int k = 0; k < C; ++k) v = fma(V[a][k] * (1.0 / lam[k]), V[b][k], v);
+          Ginv[a][b] = v;
+        }
+    } else {
+      spd_inverse_logdet<C>(G, Ginv, half_logdet);
+    }
+  }
 
   __device__ __forceinline__ void inv_metric_rows(const double (&a)[C][NV],
                                                   double (&out)[C][NV]) const {
@@ -419,7 +643,7 @@ struct ConstrainedOps {
     for (int a = 0; a < C; ++a)
 #pragma unroll
       for (int b = 0; b < C; ++b) G[a][b] = dot(J[a], W[b]);
-    spd_inverse_logdet<C>(G, Ginv, hl);
+    gram_inverse_logdet(G, Ginv, hl);
 #pragma unroll
     for (int a = 0; a < C; ++a)
 #pragma unroll
@@ -447,7 +671,7 @@ struct ConstrainedOps {
     inv_metric_vec(p, v);
 #pragma unroll
     for (int a = 0; a < C; ++a) u[a] = dot(J[a], v);
-    spd_inverse_apply<C>(G, u, w);
+    gram_solve(G, u, w);
 #pragma unroll
     for (int e = 0; e < NV; ++e) {
       double s = 0.0;
@@ -464,21 +688,14 @@ struct ConstrainedOps {
                                           double constraint_tol, double position_tol,
                                           double divergence_tol, int max_iters,
                                           int& iters) const {
-    double v[NV];
-    inv_metric_vec(p, v);
-#pragma unroll
-    for (int e = 0; e < NV; ++e) q[e] = __dadd_rn(q[e], __dmul_rn(dt, v[e]));
+    drift(q, p, dt);
     double mu[NV];
 #pragma unroll
     for (int e = 0; e < NV; ++e) mu[e] = 0.0;
     double cp[C], Jp[C][NV], S[C][NV];
     t.constr_jacob(lane, dim, q_prev, cp, Jp);
     const double adt = fabs(dt);
-    inv_metric_rows(Jp, S);
-#pragma unroll
-    for (int a = 0; a < C; ++a)
-#pragma unroll
-      for (int e = 0; e < NV; ++e) S[a][e] = adt * S[a][e];  // S_a = |dt| M^-1 Jp_a^T
+    flow_rows(Jp, adt, S);  // S_a = |dt| M^-1 Jp_a^T
     for (int i = 0; i < max_iters; ++i) {
       double c[C], J[C][NV], R[C][C], x[C];
       t.constr_jacob(lane, dim, q, c, J);
@@ -502,9 +719,7 @@ struct ConstrainedOps {
       ++iters;
       if (err > divergence_tol || err != err) return false;
       if (err < constraint_tol && maxabs(dpos) < position_tol) {
-        const double sgn = (dt > 0.0) ? 1.0 : ((dt < 0.0) ? -1.0 : 0.0);
-#pragma unroll
-        for (int e = 0; e < NV; ++e) p[e] = __dsub_rn(p[e], sgn * mu[e]);
+        finish(p, mu, dt);
         return true;
       }
 #pragma unroll
@@ -524,32 +739,31 @@ struct ConstrainedOps {
                                                        double constraint_tol, double position_tol,
                                                        double divergence_tol, int max_iters,
                                                        int& iters) const {
-    double v[NV];
-    inv_metric_vec(p, v);
-#pragma unroll
-    for (int e = 0; e < NV; ++e) q[e] = __dadd_rn(q[e], __dmul_rn(dt, v[e]));
+    drift(q, p, dt);
     double mu[NV];
 #pragma unroll
     for (int e = 0; e < NV; ++e) mu[e] = 0.0;
     double cp[C], Jp[C][NV], S[C][NV], G[C][C];
     t.constr_jacob(lane, dim, q_prev, cp, Jp);
     const double adt = fabs(dt);
-    inv_metric_rows(Jp, S);
-#pragma unroll
-    for (int a = 0; a < C; ++a)
-#pragma unroll
-      for (int e = 0; e < NV; ++e) S[a][e] = adt * S[a][e];
+    flow_rows(Jp, adt, S);
 #pragma unroll
     for (int a = 0; a < C; ++a)
 #pragma unroll
       for (int b = 0; b < C; ++b) G[a][b] = dot(Jp[a], S[b]);
+    // the Gaussian split's eigendecomposition of G, once per solve like the reference's `.inv`
+    double lam[C], V[C][C];
+    if constexpr (GAUSS) jacobi_eigh<C>(G, lam, V);
     for (int i = 0; i < max_iters; ++i) {
       double c[C], J[C][NV], x[C];
       t.constr_jacob(lane, dim, q, c, J);  // (only c is used: the Jacobian stays frozen)
       double err = 0.0;
 #pragma unroll
       for (int a = 0; a < C; ++a) err = nanmax(err, fabs(c[a]));
-      spd_inverse_apply<C>(G, c, x);
+      if constexpr (GAUSS)
+        eig_inverse_apply<C>(lam, V, c, x);
+      else
+        spd_inverse_apply<C>(G, c, x);
       double dmu[NV], dpos[NV];
 #pragma unroll
       for (int e = 0; e < NV; ++e) {
@@ -562,9 +776,7 @@ struct ConstrainedOps {
       ++iters;
       if (err > divergence_tol || err != err) return false;
       if (err < constraint_tol && maxabs(dpos) < position_tol) {
-        const double sgn = (dt > 0.0) ? 1.0 : ((dt < 0.0) ? -1.0 : 0.0);
-#pragma unroll
-        for (int e = 0; e < NV; ++e) p[e] = __dsub_rn(p[e], sgn * mu[e]);
+        finish(p, mu, dt);
         return true;
       }
 #pragma unroll
@@ -586,21 +798,14 @@ struct ConstrainedOps {
       double (&q)[NV], double (&p)[NV], const double (&q_prev)[NV], double dt,
       double constraint_tol, double position_tol, double divergence_tol, int max_iters,
       int max_ls, int& iters) const {
-    double v[NV];
-    inv_metric_vec(p, v);
-#pragma unroll
-    for (int e = 0; e < NV; ++e) q[e] = __dadd_rn(q[e], __dmul_rn(dt, v[e]));
+    drift(q, p, dt);
     double mu[NV], dpos[NV];
 #pragma unroll
     for (int e = 0; e < NV; ++e) mu[e] = 0.0, dpos[e] = 0.0;
     double cp[C], Jp[C][NV], S[C][NV];
     t.constr_jacob(lane, dim, q_prev, cp, Jp);
     const double adt = fabs(dt);
-    inv_metric_rows(Jp, S);
-#pragma unroll
-    for (int a = 0; a < C; ++a)
-#pragma unroll
-      for (int e = 0; e < NV; ++e) S[a][e] = adt * S[a][e];
+    flow_rows(Jp, adt, S);
     double step = 1.0;
     for (int i = 0; i < max_iters; ++i) {
       double c[C], J[C][NV], R[C][C], x[C];
@@ -614,9 +819,7 @@ struct ConstrainedOps {
 #pragma unroll
       for (int e = 0; e < NV; ++e) sd[e] = step * dpos[e];
       if (err < constraint_tol && (i == 0 || maxabs(sd) < position_tol)) {
-        const double sgn = (dt > 0.0) ? 1.0 : ((dt < 0.0) ? -1.0 : 0.0);
-#pragma unroll
-        for (int e = 0; e < NV; ++e) p[e] = __dsub_rn(p[e], sgn * mu[e]);
+        finish(p, mu, dt);
         return true;
       }
 #pragma unroll
@@ -669,7 +872,19 @@ struct ConstrainedOps {
   }
 };
 
-template <class Target, int KP>
+// Shared-memory doubles per warp: the rows staged by the dense metric product (C of them; the
+// Gaussian split also rotates q and p together)
+template <int C, int KP, bool GAUSS>
+__host__ __device__ constexpr int constrained_smem_per_warp() {
+  return (C > 1 ? C : (GAUSS ? 2 : 1)) * 64 * KP;
+}
+
+// GAUSS selects the flow policy of GaussianDenseConstrainedEuclideanMetricSystem
+// (systems.py:1034-1184): the h2 drift is the exact rotation, the solvers use
+// dh2_flow_dmom = (U diag(sin(w|dt|) w) U^T, U diag(cos(w|dt|)) U^T), the Gram matrices are
+// inverted through their eigendecomposition, h2 carries q.q/2 and the density is always with
+// respect to the Lebesgue measure.  omega / eigvec / eigvec_t are read only when GAUSS.
+template <class Target, int KP, bool GAUSS = false>
 __global__ void __launch_bounds__(128)
     constrained_leapfrog_kernel(const double* q_in, const double* p_in, double* q_out,
                                 double* p_out, const int32_t* __restrict__ dir, int64_t n_chains,
@@ -679,19 +894,22 @@ __global__ void __launch_bounds__(128)
                                 int max_iters, double rev_tol, double* __restrict__ h_out,
                                 int32_t* __restrict__ status, int32_t* __restrict__ n_done,
                                 int32_t* __restrict__ newton_iters, int proj_solver,
-                                int max_line_search_iters) {
+                                int max_line_search_iters, const double* __restrict__ omega,
+                                const double* __restrict__ eigvec,
+                                const double* __restrict__ eigvec_t) {
   constexpr int NV = 2 * KP;
-  constexpr int C = Target::NC;
-  constexpr int SM_PER_WARP = (C > 1 ? C : 1) * 64 * KP;
+  constexpr int SM_PER_WARP = constrained_smem_per_warp<Target::NC, KP, GAUSS>();
   extern __shared__ double smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int wpb = blockDim.x >> 5;
   const Target target(model, dim);
-  const ConstrainedOps<Target, KP> ops{target,      metric_kind,
-                                       minv,        dim,
-                                       lane,        smem + (size_t)warp * SM_PER_WARP,
-                                       proj_solver, max_line_search_iters};
+  ConstrainedOps<Target, KP, GAUSS> ops{target,      metric_kind,
+                                        minv,        dim,
+                                        lane,        smem + (size_t)warp * SM_PER_WARP,
+                                        proj_solver, max_line_search_iters,
+                                        omega,       eigvec,
+                                        eigvec_t};
   const bool even = (dim & 1) == 0;
 
   for (int64_t ch = (int64_t)blockIdx.x * wpb + warp; ch < n_chains;
@@ -717,13 +935,15 @@ __global__ void __launch_bounds__(128)
       }
       q[2 * k] = q0, q[2 * k + 1] = q1, p[2 * k] = p0, p[2 * k + 1] = p1;
     }
-    const bool lebesgue = model.tp[MB200_MAX_PARAMS - 1] != 0.0;  // dens_wrt_hausdorff=False
+    // dens_wrt_hausdorff=False
+    const bool lebesgue = GAUSS || model.tp[MB200_MAX_PARAMS - 1] != 0.0;
     ops.dh1(q, g, lebesgue);
     int st = MB200_STATUS_OK, done = 0, iters = 0;
     // constraint-Jacobian evaluations: one per projection, one per retraction (at the previous
     // position) plus one per Newton iteration, one per Lebesgue-density gradient
     int n_proj = 0, n_retr = 0;
     const double dt_inner = dt / n_inner;
+    if constexpr (GAUSS) ops.set_rotation(fabs(dt_inner));
     for (int s = 0; s < ns && st == MB200_STATUS_OK; ++s) {
       double qs[NV], ps[NV];
 #pragma unroll
@@ -797,7 +1017,12 @@ __global__ void __launch_bounds__(128)
         ops.dh1(q, gtmp, true, &ldsg);
         l += ldsg;
       }
-      if (lane == 0) h_out[ch] = l + 0.5 * kin;
+      if constexpr (GAUSS) {  // h1 + (q.q/2 + p.M^-1 p/2) (systems.py:451-454)
+        const double qq = ConstrainedOps<Target, KP>::dot(q, q);
+        if (lane == 0) h_out[ch] = l + (0.5 * qq + 0.5 * kin);
+      } else {
+        if (lane == 0) h_out[ch] = l + 0.5 * kin;
+      }
     }
     if (lane == 0) {
       if (status != nullptr) status[ch] = st;
@@ -816,21 +1041,21 @@ __global__ void __launch_bounds__(128)
 // Projection of momenta onto the cotangent space of the constraint manifold for all chains:
 // ConstrainedTractableFlowSystem.sample_momentum (systems.py:613-616) draws from N(0, M) and
 // then applies project_onto_cotangent_space (systems.py:863-873); this is that second half.
-template <class Target, int KP>
+// GAUSS: the Gram matrix is inverted through its eigendecomposition (systems.py:1157-1169).
+template <class Target, int KP, bool GAUSS = false>
 __global__ void __launch_bounds__(128)
     constrained_project_kernel(const double* __restrict__ q_in, const double* p_in, double* p_out,
                                int64_t n_chains, int dim, int metric_kind,
                                const double* __restrict__ minv, ModelArgs model) {
   constexpr int NV = 2 * KP;
-  constexpr int C = Target::NC;
-  constexpr int SM_PER_WARP = (C > 1 ? C : 1) * 64 * KP;
+  constexpr int SM_PER_WARP = constrained_smem_per_warp<Target::NC, KP, GAUSS>();
   extern __shared__ double smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int wpb = blockDim.x >> 5;
   const Target target(model, dim);
-  const ConstrainedOps<Target, KP> ops{target, metric_kind, minv, dim, lane,
-                                       smem + (size_t)warp * SM_PER_WARP, 0, 0};
+  const ConstrainedOps<Target, KP, GAUSS> ops{target, metric_kind, minv, dim, lane,
+                                              smem + (size_t)warp * SM_PER_WARP, 0, 0};
   for (int64_t ch = (int64_t)blockIdx.x * wpb + warp; ch < n_chains;
        ch += (int64_t)gridDim.x * wpb) {
     double q[NV], p[NV];

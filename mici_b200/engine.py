@@ -18,6 +18,9 @@ def build_system(problem):
         return systems.DenseConstrainedEuclideanMetricSystem(
             target, target, metric=problem.metric,
             dens_wrt_hausdorff=problem.system_kwargs.get("dens_wrt_hausdorff", True))
+    if problem.system == "gaussian_constrained_euclidean":
+        return systems.GaussianDenseConstrainedEuclideanMetricSystem(
+            target, target, metric=problem.metric)
     if problem.system == "softabs_riemannian":
         return systems.SoftAbsRiemannianMetricSystem(target, **problem.system_kwargs)
     if problem.system == "dense_riemannian":

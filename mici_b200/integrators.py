@@ -45,6 +45,7 @@ from .states import ChainState
 from .systems import (
     ConstrainedEuclideanMetricSystem,
     EuclideanMetricSystem,
+    GaussianDenseConstrainedEuclideanMetricSystem,
     GaussianEuclideanMetricSystem,
     RiemannianMetricSystem,
     _batched,
@@ -521,7 +522,9 @@ class ImplicitMidpointIntegrator(_ImplicitIntegrator):
 
 class ConstrainedLeapfrogIntegrator(TractableFlowIntegrator):
     """Leapfrog for constrained systems: RATTLE / geodesic integrator with Newton projection
-    and reversibility check (integrators.py:684-984)."""
+    and reversibility check (integrators.py:684-984).  A
+    ``GaussianDenseConstrainedEuclideanMetricSystem`` runs through its own entry point, whose
+    drift is the exact rotation of the Gaussian split."""
 
     def __init__(self, system, step_size=None, n_inner_step=1, reverse_check_tol=2e-8,
                  reverse_check_norm=maximum_norm,
@@ -549,14 +552,21 @@ class ConstrainedLeapfrogIntegrator(TractableFlowIntegrator):
         model = sysm._model(dev)
         eps, eps_t, ns, max_n = _step_args(self.step_size, n_steps, n, dev)
         iters = torch.zeros(n, dtype=torch.int32, device=dev)
-        rc = _lib.load().mb200_constrained_leapfrog_euclidean(
+        metric = (sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(dev)))
+        if isinstance(sysm, GaussianDenseConstrainedEuclideanMetricSystem):
+            # exact h2 rotation with per-chain sin / cos, eigh-inverted Gram matrices
+            entry = "mb200_constrained_leapfrog_gaussian_euclidean"
+            metric += tuple(_lib.ptr(a) for a in sysm.rotation_args(dev))
+        else:
+            entry = "mb200_constrained_leapfrog_euclidean"
+        rc = getattr(_lib.load(), entry)(
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
             n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), int(self.n_inner_step),
-            sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model),
+            *metric, ctypes.byref(model),
             self.projection_solver.kind, float(kw["constraint_tol"]), float(kw["position_tol"]),
             float(kw["divergence_tol"]), int(kw["max_iters"]),
             int(kw.get("max_line_search_iters", 10)), float(self.reverse_check_tol), _lib.ptr(h),
             _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters), _lib.current_stream_ptr(dev),
         )
-        _lib.check(rc, "mb200_constrained_leapfrog_euclidean")
+        _lib.check(rc, entry)
         return iters

@@ -24,7 +24,7 @@ class Problem:
         integrator: ``"leapfrog"`` | ``"implicit_leapfrog"`` | ``"constrained_leapfrog"``.
         system: ``"euclidean"`` | ``"softabs_riemannian"`` | ``"dense_riemannian"`` |
             ``"diagonal_riemannian"`` | ``"scalar_riemannian"`` | ``"cholesky_riemannian"`` |
-            ``"constrained_euclidean"``.
+            ``"constrained_euclidean"`` | ``"gaussian_constrained_euclidean"``.
         target: target-model name (``mici_b200.targets`` registry key).
         target_params: constructor kwargs of the target model.
         metric: ``None`` (identity), 1-D (diagonal) or 2-D (dense SPD) array -- the fixed
@@ -423,6 +423,22 @@ def multi_sphere_constrained(n_chains=32, dim=16, n_constr=4, seed=BASE_SEED + 8
     )
 
 
+def c9_gaussian_constrained(n_chains=8192, dim=128, n_constr=8, seed=BASE_SEED + 12,
+                            step_size=0.1):
+    """C9: GaussianDenseConstrainedEuclideanMetricSystem on the multi-sphere target, C = 8,
+    D = 128, dense metric, Newton projection; start states on the manifold with projected momenta
+    as in ``multi_sphere_constrained``.  Step size 0.1, chosen on the CPU oracle: every step of the
+    reference fixture at this shape (gc_multi_sphere_c8_dense_d128, 3 chains, 5 steps) and of the
+    C = 8, D = 32 fixture (8 chains, 20 steps) converges."""
+    base = multi_sphere_constrained(n_chains=n_chains, dim=dim, n_constr=n_constr, seed=seed,
+                                    metric_kind="dense")
+    base.name = "C9"
+    base.system = "gaussian_constrained_euclidean"
+    base.system_kwargs = {}
+    base.step_size = step_size
+    return base
+
+
 CONFIGS = {
     "C0": c0_std_gaussian,
     "C1": c1_funnel,
@@ -433,6 +449,7 @@ CONFIGS = {
     "C6": c6_softabs_quartic,
     "C7": c7_funnel_riemannian,
     "C8": c8_cholesky_riemannian,
+    "C9": c9_gaussian_constrained,
     "S1": sphere_constrained,
     "S2": multi_sphere_constrained,
     "G1": g1_gaussian_split,

@@ -4,6 +4,7 @@ hot path:
 
 * ``EuclideanMetricSystem``                   systems.py:264-366
 * ``DenseConstrainedEuclideanMetricSystem``   systems.py:619-873, 876-1031
+* ``GaussianDenseConstrainedEuclideanMetricSystem``  systems.py:1034-1184
 * ``DenseRiemannianMetricSystem``             systems.py:1187-1402, 1710-1760
 * ``SoftAbsRiemannianMetricSystem``           systems.py:1763-1920
 * ``ScalarRiemannianMetricSystem``            systems.py:1405-1490
@@ -474,6 +475,9 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
     def project_onto_cotangent_space(self, mom, state):
         """``mom - J^T (J M^-1 J^T)^-1 J M^-1 mom`` at ``state.pos`` (systems.py:863-873) for all
         chains in one launch (``mb200_project_onto_cotangent_space``)."""
+        return self._project(mom, state, "mb200_project_onto_cotangent_space")
+
+    def _project(self, mom, state, entry):
         pos = state.pos
         single = pos.ndim == 1
         ref = mom
@@ -489,11 +493,11 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
         m = self._metric
         minv = None if m.kind == METRIC_IDENTITY else m.inv_device(dev)
         model = self._model(dev)
-        rc = _lib.load().mb200_project_onto_cotangent_space(
+        rc = getattr(_lib.load(), entry)(
             _lib.ptr(pos_t), _lib.ptr(mom_t), _lib.ptr(out), n, dim, m.kind, _lib.ptr(minv),
             ctypes.byref(model), _lib.current_stream_ptr(dev),
         )
-        _lib.check(rc, "mb200_project_onto_cotangent_space")
+        _lib.check(rc, entry)
         return _like_input(ref, out[0] if single else out)
 
 
@@ -508,6 +512,82 @@ class DenseConstrainedEuclideanMetricSystem(ConstrainedEuclideanMetricSystem):
                          dens_wrt_hausdorff=dens_wrt_hausdorff,
                          grad_neg_log_dens=grad_neg_log_dens, jacob_constr=jacob_constr,
                          backend=backend)
+
+
+class GaussianDenseConstrainedEuclideanMetricSystem(GaussianEuclideanMetricSystem,
+                                                    DenseConstrainedEuclideanMetricSystem):
+    """Gaussian Euclidean system subject to a dense set of constraints (systems.py:1034-1184):
+    the target density is relative to the standard Gaussian measure on the ambient space and is
+    conditioned on ``constr(q) == 0`` (always ``dens_wrt_hausdorff=False``).  ``h1 = l(q) +
+    log det gram / 2``, ``h2 = q.q/2 + p.M^-1 p/2`` whose flow is the exact rotation in the
+    eigenbasis of ``M``; the Gram matrices are inverted through their eigendecomposition.  The
+    constrained leapfrog drives it through ``mb200_constrained_leapfrog_gaussian_euclidean``."""
+
+    def __init__(self, neg_log_dens, constr=None, *, metric=None, grad_neg_log_dens=None,
+                 jacob_constr=None, mhp_constr=None, backend=None):
+        DenseConstrainedEuclideanMetricSystem.__init__(
+            self, neg_log_dens, constr, metric=metric, dens_wrt_hausdorff=False,
+            grad_neg_log_dens=grad_neg_log_dens, jacob_constr=jacob_constr,
+            mhp_constr=mhp_constr, backend=backend)
+
+    def rotation_args(self, device):
+        """Device operands ``(metric_omega, metric_eigvec, metric_eigvec_t)`` of
+        ``mb200_constrained_leapfrog_gaussian_euclidean``: ``w = 1 / eigval**0.5`` computed as
+        the reference does (systems.py:1176), and ``U``, ``U^T`` for a dense metric."""
+        m = self._metric
+        key = ("gauss_constr", str(device))
+        if key not in m._dev:
+            dim = self.target.dim
+            if m.kind == METRIC_IDENTITY:
+                omega, u = 1.0 / np.ones(dim) ** 0.5, None
+            elif m.kind == METRIC_DIAGONAL:
+                omega, u = 1.0 / m.array**0.5, None
+            else:
+                eigval, u = self._eig()
+                omega = 1.0 / eigval**0.5
+            m._dev[key] = tuple(
+                None if a is None else torch.as_tensor(np.ascontiguousarray(a), device=device)
+                for a in (omega, u, None if u is None else u.T))
+        return m._dev[key]
+
+    def h(self, state):
+        """``h1 + h2`` (systems.py:187-196, 451-454, 853-856), evaluated by a zero-step launch of
+        the Gaussian constrained kernel."""
+        pos, mom, _, single = _batched(state)
+        n, dim = pos.shape
+        dev = pos.device
+        pos, mom = pos.contiguous(), mom.contiguous()
+        h = torch.empty(n, dtype=torch.float64, device=dev)
+        scratch_q, scratch_p = torch.empty_like(pos), torch.empty_like(mom)
+        m = self._metric
+        om, u, ut = self.rotation_args(dev)
+        rc = _lib.load().mb200_constrained_leapfrog_gaussian_euclidean(
+            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(scratch_q), _lib.ptr(scratch_p), None, n, dim,
+            0.0, None, 0, None, 1, m.kind, _lib.ptr(m.inv_device(dev)), _lib.ptr(om), _lib.ptr(u),
+            _lib.ptr(ut), ctypes.byref(self._model(dev)), 0, 1e-9, 1e-8, 1e10, 50, 10, 2e-8,
+            _lib.ptr(h), None, None, None, _lib.current_stream_ptr(dev),
+        )
+        _lib.check(rc, "mb200_constrained_leapfrog_gaussian_euclidean")
+        return _like_input(state.pos, h[0] if single else h)
+
+    def h2(self, state):
+        """``q.q/2 + p.M^-1 p/2`` (systems.py:451-454)."""
+        return GaussianEuclideanMetricSystem.h2(self, state)
+
+    def dh2_dpos(self, state):
+        """systems.py:460-462."""
+        return state.pos
+
+    def h2_flow(self, state, dt):
+        raise NotImplementedError(
+            "The exact h2 flow of a constrained Gaussian system runs inside the constrained "
+            "leapfrog kernel, followed by the projection onto the manifold.")
+
+    def project_onto_cotangent_space(self, mom, state):
+        """``mom - J^T gram^-1 (J M^-1 mom)`` with ``gram`` a ``DenseSymmetricMatrix`` inverted
+        through its eigendecomposition (systems.py:863-873, 1157-1169), all chains in one launch
+        (``mb200_project_onto_cotangent_space_gaussian``)."""
+        return self._project(mom, state, "mb200_project_onto_cotangent_space_gaussian")
 
 
 class RiemannianMetricSystem(System):
