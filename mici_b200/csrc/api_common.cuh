@@ -106,16 +106,45 @@ int leapfrog_dmma_dispatch(const double* q_in, const double* p_in, double* q_out
                            double eps, int n_steps, const double* minv, const ModelArgs& m,
                            double* h_out, int32_t* status, int32_t* n_done, cudaStream_t st);
 
-// implemented in api_dense.cu (global-workspace dense metric policy, dense_global.cuh)
+// Arguments of one implicit-integrator launch on a Riemannian system (leapfrog or midpoint steps;
+// zero steps evaluate the Hamiltonian only).  ws / ws_bytes: the caller's workspace, or NULL.
+struct ImplicitArgs {
+  const double *q_in, *p_in;
+  double *q_out, *p_out;
+  const int32_t* dir;
+  int64_t n;
+  int dim;
+  double eps;
+  int n_steps;
+  ModelArgs m;
+  double fp_tol, fp_div;
+  int fp_max;
+  double rev_tol;
+  double* h_out;
+  int32_t *status, *n_done, *fp_iters;
+  int fp_solver;
+  void* ws;
+  int64_t ws_bytes;
+  cudaStream_t st;
+};
+
+// Arguments of one per-chain metric-vector product on a Riemannian system: sqrt(M(q)) v
+// (momentum refresh) or M(q)^-1 v (velocity)
+struct VectorArgs {
+  const double *q, *v;
+  double* out;
+  int64_t n;
+  int dim;
+  ModelArgs m;
+  int32_t* status;
+  cudaStream_t st;
+};
+
+// implemented in api_dense.cu (global-workspace dense metric policy, dense_global.cuh); the
+// route to it is decided, and its arguments checked, in api_riemannian.cu
 int64_t dense_global_workspace_bytes(int64_t n_chains, int dim);
 bool dense_global_supported(int dim);
-int dense_global_implicit(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                          const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
-                          const ModelArgs& m, double fp_tol, double fp_div, int fp_max,
-                          double rev_tol, double* h_out, int32_t* status, int32_t* n_done,
-                          int32_t* fp_iters, cudaStream_t st, int midpoint, int fp_solver, void* ws,
-                          int64_t ws_bytes);
-int dense_global_vector(const double* q, const double* v, double* out, int64_t n, int dim,
-                        const ModelArgs& m, int32_t* status, cudaStream_t st, int velocity);
+int dense_global_implicit(const ImplicitArgs& a, bool hadamard);
+int dense_global_vector(const VectorArgs& a, bool velocity, bool hadamard);
 
 }  // namespace mb200

@@ -12,46 +12,60 @@ struct GaussianArgs {
   const double* eigvec_t;
 };
 
-template <bool GAUSS, class Target, int KP>
-static int launch_constrained(const double* q_in, const double* p_in, double* q_out,
-                              double* p_out, const int32_t* dir, int64_t n, int dim, double eps,
-                              int n_steps, int n_inner, int metric_kind, const double* minv,
-                              const ModelArgs& m, double ctol, double ptol, double dtol,
-                              int max_iters, double rev_tol, double* h_out, int32_t* status,
-                              int32_t* n_done, int32_t* iters, cudaStream_t st, int proj_solver,
-                              int max_ls, const GaussianArgs& ga) {
-  constexpr int WARPS = 4;
-  auto kern = constrained_leapfrog_kernel<Target, KP, GAUSS>;
-  const size_t smem =
-      (size_t)WARPS * constrained_smem_per_warp<Target::NC, KP, GAUSS>() * sizeof(double);
-  int64_t blocks = (n + WARPS - 1) / WARPS;
+constexpr int CS_WARPS = 4;  // chains (one warp each) per CTA of the warp-per-chain kernels
+
+// CTAs for n chains at `per_cta` chains per CTA, at most 16 per SM (grid-stride loop beyond)
+static unsigned cs_blocks(int64_t n, int per_cta) {
+  int64_t blocks = (n + per_cta - 1) / per_cta;
   const int64_t cap = (int64_t)num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  kern<<<(unsigned)blocks, WARPS * 32, smem, st>>>(q_in, p_in, q_out, p_out, dir, n, dim, eps,
-                                                   n_steps, n_inner, metric_kind, minv, m, ctol,
-                                                   ptol, dtol, max_iters, rev_tol, h_out, status,
-                                                   n_done, iters, proj_solver, max_ls, ga.omega,
-                                                   ga.eigvec, ga.eigvec_t);
-  return check_launch("constrained_leapfrog_kernel");
+  return (unsigned)(blocks > cap ? cap : blocks);
 }
 
-template <bool GAUSS, class Target, int KP>
-static int launch_project(const double* q, const double* p_in, double* p_out, int64_t n, int dim,
-                          int metric_kind, const double* minv, const ModelArgs& m,
-                          cudaStream_t st) {
-  constexpr int WARPS = 4;
-  const size_t smem =
-      (size_t)WARPS * constrained_smem_per_warp<Target::NC, KP, GAUSS>() * sizeof(double);
-  int64_t blocks = (n + WARPS - 1) / WARPS;
-  const int64_t cap = (int64_t)num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  constrained_project_kernel<Target, KP, GAUSS><<<(unsigned)blocks, WARPS * 32, smem, st>>>(
-      q, p_in, p_out, n, dim, metric_kind, minv, m);
-  return check_launch("constrained_project_kernel");
+// A constrained target and its per-lane element count KP, as the dispatch below hands them over
+template <class T, int KP_>
+struct CsShape {
+  using Target = T;
+  static constexpr int KP = KP_;
+  template <bool GAUSS>
+  static size_t smem() {
+    return (size_t)CS_WARPS * constrained_smem_per_warp<T::NC, KP, GAUSS>() * sizeof(double);
+  }
+};
+
+// Target / size dispatch shared by the constrained entry points: `launch(CsShape<Target, KP>{})`
+// starts the operation's kernel
+template <class Launch>
+static int constrained_target_dispatch(const ModelArgs& m, int dim, const Launch& launch) {
+  switch (m.target_id) {
+    case MB200_TARGET_TORUS:
+      if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
+      return launch(CsShape<TorusTarget, 1>{});
+    case MB200_TARGET_SPHERE:
+      if (dim <= 64) return launch(CsShape<SphereTarget, 1>{});
+      if (dim <= 128) return launch(CsShape<SphereTarget, 2>{});
+      if (dim <= 256) return launch(CsShape<SphereTarget, 4>{});
+      return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
+    case MB200_TARGET_MULTI_SPHERE: {
+      const int nc = (int)m.tp[0];
+      if ((nc != 2 && nc != 4 && nc != 8) || dim % nc != 0 || dim > 128)
+        return fail(MB200_ERR_UNSUPPORTED,
+                    "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
+      if (dim <= 64) {
+        if (nc == 2) return launch(CsShape<MultiSphereTarget<2>, 1>{});
+        if (nc == 4) return launch(CsShape<MultiSphereTarget<4>, 1>{});
+        return launch(CsShape<MultiSphereTarget<8>, 1>{});
+      }
+      if (nc == 2) return launch(CsShape<MultiSphereTarget<2>, 2>{});
+      if (nc == 4) return launch(CsShape<MultiSphereTarget<4>, 2>{});
+      return launch(CsShape<MultiSphereTarget<8>, 2>{});
+    }
+    default:
+      return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
+  }
 }
 
-// Argument checks and target / size dispatch shared by the plain and the Gaussian-split entry
-// points (the torus one-thread kernel serves the plain system's Hausdorff density only).
+// Argument checks shared by the plain and the Gaussian-split entry points (the torus one-thread
+// kernel serves the plain system's Hausdorff density only).
 template <bool GAUSS>
 static int constrained_leapfrog_dispatch(
     const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
@@ -79,53 +93,29 @@ static int constrained_leapfrog_dispatch(
   const DeviceScope device_scope(pos_in);
   const ModelArgs m = to_args(model, step_sizes, n_steps_per_chain);
   cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS                                                                              \
-  pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps, n_inner_step,       \
-      metric_kind, metric_inv, m, constraint_tol, position_tol, divergence_tol, max_iters,      \
-      reverse_check_tol, h_out, status, n_done, newton_iters, st, projection_solver,            \
-      max_line_search_iters, ga
-  switch (m.target_id) {
-    case MB200_TARGET_TORUS:
-      if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
-      // config C3: identity metric, Newton projection, Hausdorff density -> one THREAD per chain
-      if (!GAUSS && metric_kind == MB200_METRIC_IDENTITY &&
-          projection_solver == MB200_PROJ_SOLVER_NEWTON && m.tp[MB200_MAX_PARAMS - 1] == 0.0) {
-        // latency bound per chain: spread small batches over as many warps as there are
-        // sub-partitions (measured: 8 lanes per warp 0.287 ms, 32 lanes 0.300 ms at 4096 chains)
-        const int lanes = n_chains >= (int64_t)num_sms() * 4 * 32 ? 32 : 8;
-        int64_t blocks = (n_chains + lanes - 1) / lanes;
-        const int64_t cap = (int64_t)num_sms() * 16;
-        if (blocks > cap) blocks = cap;
-        constrained_torus_thread_kernel<<<(unsigned)blocks, 32, 0, st>>>(
-            pos_in, mom_in, pos_out, mom_out, dir, n_chains, step_size, n_steps, n_inner_step, m,
-            constraint_tol, position_tol, divergence_tol, max_iters, reverse_check_tol, h_out,
-            status, n_done, newton_iters, lanes);
-        return check_launch("constrained_torus_thread_kernel");
-      }
-      return launch_constrained<GAUSS, TorusTarget, 1>(MB200_ARGS);
-    case MB200_TARGET_SPHERE:
-      if (dim <= 64) return launch_constrained<GAUSS, SphereTarget, 1>(MB200_ARGS);
-      if (dim <= 128) return launch_constrained<GAUSS, SphereTarget, 2>(MB200_ARGS);
-      if (dim <= 256) return launch_constrained<GAUSS, SphereTarget, 4>(MB200_ARGS);
-      return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
-    case MB200_TARGET_MULTI_SPHERE: {
-      const int nc = (int)m.tp[0];
-      if ((nc != 2 && nc != 4 && nc != 8) || dim % nc != 0 || dim > 128)
-        return fail(MB200_ERR_UNSUPPORTED,
-                    "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
-      if (dim <= 64) {
-        if (nc == 2) return launch_constrained<GAUSS, MultiSphereTarget<2>, 1>(MB200_ARGS);
-        if (nc == 4) return launch_constrained<GAUSS, MultiSphereTarget<4>, 1>(MB200_ARGS);
-        return launch_constrained<GAUSS, MultiSphereTarget<8>, 1>(MB200_ARGS);
-      }
-      if (nc == 2) return launch_constrained<GAUSS, MultiSphereTarget<2>, 2>(MB200_ARGS);
-      if (nc == 4) return launch_constrained<GAUSS, MultiSphereTarget<4>, 2>(MB200_ARGS);
-      return launch_constrained<GAUSS, MultiSphereTarget<8>, 2>(MB200_ARGS);
-    }
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
+  // config C3: torus, identity metric, Newton projection, Hausdorff density -> one THREAD per chain
+  if (!GAUSS && m.target_id == MB200_TARGET_TORUS && dim == 3 &&
+      metric_kind == MB200_METRIC_IDENTITY && projection_solver == MB200_PROJ_SOLVER_NEWTON &&
+      m.tp[MB200_MAX_PARAMS - 1] == 0.0) {
+    // latency bound per chain: spread small batches over as many warps as there are
+    // sub-partitions (measured: 8 lanes per warp 0.287 ms, 32 lanes 0.300 ms at 4096 chains)
+    const int lanes = n_chains >= (int64_t)num_sms() * 4 * 32 ? 32 : 8;
+    constrained_torus_thread_kernel<<<cs_blocks(n_chains, lanes), 32, 0, st>>>(
+        pos_in, mom_in, pos_out, mom_out, dir, n_chains, step_size, n_steps, n_inner_step, m,
+        constraint_tol, position_tol, divergence_tol, max_iters, reverse_check_tol, h_out, status,
+        n_done, newton_iters, lanes);
+    return check_launch("constrained_torus_thread_kernel");
   }
-#undef MB200_ARGS
+  return constrained_target_dispatch(m, dim, [&](auto shape) {
+    using S = decltype(shape);
+    constrained_leapfrog_kernel<typename S::Target, S::KP, GAUSS>
+        <<<cs_blocks(n_chains, CS_WARPS), CS_WARPS * 32, S::template smem<GAUSS>(), st>>>(
+            pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps,
+            n_inner_step, metric_kind, metric_inv, m, constraint_tol, position_tol,
+            divergence_tol, max_iters, reverse_check_tol, h_out, status, n_done, newton_iters,
+            projection_solver, max_line_search_iters, ga.omega, ga.eigvec, ga.eigvec_t);
+    return check_launch("constrained_leapfrog_kernel");
+  });
 }
 
 template <bool GAUSS>
@@ -140,35 +130,13 @@ static int project_dispatch(const double* pos, const double* mom_in, double* mom
     return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
   const DeviceScope device_scope(pos);
   const ModelArgs m = to_args(model);
-  cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv, m, st
-  switch (m.target_id) {
-    case MB200_TARGET_TORUS:
-      if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
-      return launch_project<GAUSS, TorusTarget, 1>(MB200_ARGS);
-    case MB200_TARGET_SPHERE:
-      if (dim <= 64) return launch_project<GAUSS, SphereTarget, 1>(MB200_ARGS);
-      if (dim <= 128) return launch_project<GAUSS, SphereTarget, 2>(MB200_ARGS);
-      if (dim <= 256) return launch_project<GAUSS, SphereTarget, 4>(MB200_ARGS);
-      return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
-    case MB200_TARGET_MULTI_SPHERE: {
-      const int nc = (int)m.tp[0];
-      if ((nc != 2 && nc != 4 && nc != 8) || dim % nc != 0 || dim > 128)
-        return fail(MB200_ERR_UNSUPPORTED,
-                    "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
-      if (dim <= 64) {
-        if (nc == 2) return launch_project<GAUSS, MultiSphereTarget<2>, 1>(MB200_ARGS);
-        if (nc == 4) return launch_project<GAUSS, MultiSphereTarget<4>, 1>(MB200_ARGS);
-        return launch_project<GAUSS, MultiSphereTarget<8>, 1>(MB200_ARGS);
-      }
-      if (nc == 2) return launch_project<GAUSS, MultiSphereTarget<2>, 2>(MB200_ARGS);
-      if (nc == 4) return launch_project<GAUSS, MultiSphereTarget<4>, 2>(MB200_ARGS);
-      return launch_project<GAUSS, MultiSphereTarget<8>, 2>(MB200_ARGS);
-    }
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
-  }
-#undef MB200_ARGS
+  return constrained_target_dispatch(m, dim, [&](auto shape) {
+    using S = decltype(shape);
+    constrained_project_kernel<typename S::Target, S::KP, GAUSS>
+        <<<cs_blocks(n_chains, CS_WARPS), CS_WARPS * 32, S::template smem<GAUSS>(),
+           (cudaStream_t)stream>>>(pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv, m);
+    return check_launch("constrained_project_kernel");
+  });
 }
 
 }  // namespace mb200

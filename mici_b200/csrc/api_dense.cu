@@ -20,92 +20,50 @@ bool dense_global_supported(int dim) {
   return rm_smem_doubles(dim, RM_NMATS_GLOBAL) * sizeof(double) <= 227 * 1024;
 }
 
-template <class Target, template <class> class MetricT>
-static int dg_launch_implicit(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                              const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
-                              ModelArgs m, double fp_tol, double fp_div, int fp_max, double rev_tol,
-                              double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
-                              cudaStream_t st, int fp_solver, void* ws, int64_t ws_bytes) {
-  auto kern = implicit_leapfrog_kernel<Target, MetricT>;
-  const size_t smem = rm_smem_doubles(dim, RM_NMATS_GLOBAL) * sizeof(double);
+template <template <class> class MetricT>
+static int dg_launch_implicit(const ImplicitArgs& a) {
+  auto kern = implicit_leapfrog_kernel<QuadraticRTarget, MetricT>;
+  const size_t smem = rm_smem_doubles(a.dim, RM_NMATS_GLOBAL) * sizeof(double);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  const int blocks = dg_blocks(n);
-  DgScratch scratch(ws, ws_bytes, (size_t)dense_global_workspace_bytes(n, dim), st);
+  const int blocks = dg_blocks(a.n);
+  DgScratch scratch(a.ws, a.ws_bytes, (size_t)dense_global_workspace_bytes(a.n, a.dim), a.st);
   if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "dense metric workspace allocation failed");
+  ModelArgs m = a.m;
   m.workspace = scratch.ptr;
-  m.ws_stride = dg_workspace_doubles(dim);
-  kern<<<(unsigned)blocks, DG_THREADS, smem, st>>>(q_in, p_in, q_out, p_out, dir, n, dim, eps,
-                                                   n_steps, m, fp_tol, fp_div, fp_max, rev_tol,
-                                                   h_out, status, n_done, fp_iters,
-                                                   RM_NMATS_GLOBAL, 0, fp_solver);
+  m.ws_stride = dg_workspace_doubles(a.dim);
+  kern<<<(unsigned)blocks, DG_THREADS, smem, a.st>>>(
+      a.q_in, a.p_in, a.q_out, a.p_out, a.dir, a.n, a.dim, a.eps, a.n_steps, m, a.fp_tol, a.fp_div,
+      a.fp_max, a.rev_tol, a.h_out, a.status, a.n_done, a.fp_iters, RM_NMATS_GLOBAL, 0, a.fp_solver);
   return check_launch("implicit_leapfrog_kernel (global dense metric)");
 }
 
-int dense_global_implicit(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                          const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
-                          const ModelArgs& m, double fp_tol, double fp_div, int fp_max,
-                          double rev_tol, double* h_out, int32_t* status, int32_t* n_done,
-                          int32_t* fp_iters, cudaStream_t st, int midpoint, int fp_solver, void* ws,
-                          int64_t ws_bytes) {
-  if (midpoint)
-    return fail(MB200_ERR_UNSUPPORTED,
-                "implicit midpoint is not available for the global-workspace dense metric");
-  if (!dense_global_supported(dim))
-    return fail(MB200_ERR_UNSUPPORTED, "dim %d: panel buffers exceed shared memory", dim);
-  if (!m.maux) return fail(MB200_ERR_INVALID_ARG, "dense metric needs its matrices (rmetric_aux)");
-  if (m.target_id != MB200_TARGET_QUADRATIC)
-    return fail(MB200_ERR_UNSUPPORTED,
-                "target %d not compiled for the global-workspace dense metric", m.target_id);
-  if (!m.taux) return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
-#define MB200_ARGS                                                                         \
-  q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, m, fp_tol, fp_div, fp_max, rev_tol, \
-      h_out, status, n_done, fp_iters, st, fp_solver, ws, ws_bytes
-  if (m.rmetric_id == MB200_RMETRIC_HADAMARD)
-    return dg_launch_implicit<QuadraticRTarget, GlobalDenseHadamard>(MB200_ARGS);
-  return dg_launch_implicit<QuadraticRTarget, GlobalDenseRank1>(MB200_ARGS);
-#undef MB200_ARGS
+int dense_global_implicit(const ImplicitArgs& a, bool hadamard) {
+  return hadamard ? dg_launch_implicit<GlobalDenseHadamard>(a) : dg_launch_implicit<GlobalDenseRank1>(a);
 }
 
-template <class Target, template <class> class MetricT, bool VELOCITY>
-static int dg_launch_vec(const double* q, const double* v, double* out, int64_t n, int dim,
-                         ModelArgs m, int32_t* status, cudaStream_t st) {
-  const size_t smem = rm_smem_doubles(dim, RM_NMATS_GLOBAL) * sizeof(double);
-  const int blocks = dg_blocks(n);
-  DgScratch scratch(nullptr, 0, (size_t)dense_global_workspace_bytes(n, dim), st);
+template <template <class> class MetricT, bool VELOCITY>
+static int dg_launch_vec(const VectorArgs& a) {
+  const size_t smem = rm_smem_doubles(a.dim, RM_NMATS_GLOBAL) * sizeof(double);
+  const int blocks = dg_blocks(a.n);
+  DgScratch scratch(nullptr, 0, (size_t)dense_global_workspace_bytes(a.n, a.dim), a.st);
   if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "dense metric workspace allocation failed");
+  ModelArgs m = a.m;
   m.workspace = scratch.ptr;
-  m.ws_stride = dg_workspace_doubles(dim);
-  cudaError_t e;
-  if (VELOCITY) {
-    auto kern = riemannian_velocity_kernel<Target, MetricT>;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-    kern<<<(unsigned)blocks, DG_THREADS, smem, st>>>(q, v, out, n, dim, m, status, RM_NMATS_GLOBAL);
-  } else {
-    auto kern = riemannian_sample_momentum_kernel<Target, MetricT>;
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-    kern<<<(unsigned)blocks, DG_THREADS, smem, st>>>(q, v, out, n, dim, m, status, RM_NMATS_GLOBAL);
-  }
+  m.ws_stride = dg_workspace_doubles(a.dim);
+  auto kern = riemannian_vector_kernel<QuadraticRTarget, MetricT, VELOCITY>();
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
+  kern<<<(unsigned)blocks, DG_THREADS, smem, a.st>>>(a.q, a.v, a.out, a.n, a.dim, m, a.status,
+                                                     RM_NMATS_GLOBAL);
   return check_launch("riemannian vector kernel (global dense metric)");
 }
 
-// velocity = 1: out = M(q)^-1 v ; velocity = 0: out = chol(M(q)) v
-int dense_global_vector(const double* q, const double* v, double* out, int64_t n, int dim,
-                        const ModelArgs& m, int32_t* status, cudaStream_t st, int velocity) {
-  if (!dense_global_supported(dim))
-    return fail(MB200_ERR_UNSUPPORTED, "dim %d: panel buffers exceed shared memory", dim);
-  if (!m.maux) return fail(MB200_ERR_INVALID_ARG, "dense metric needs its matrices (rmetric_aux)");
-  if (m.target_id != MB200_TARGET_QUADRATIC)
-    return fail(MB200_ERR_UNSUPPORTED,
-                "target %d not compiled for the global-workspace dense metric", m.target_id);
-  const bool had = m.rmetric_id == MB200_RMETRIC_HADAMARD;
+// velocity: out = M(q)^-1 v ; else out = chol(M(q)) v
+int dense_global_vector(const VectorArgs& a, bool velocity, bool hadamard) {
   if (velocity)
-    return had ? dg_launch_vec<QuadraticRTarget, GlobalDenseHadamard, true>(q, v, out, n, dim, m, status, st)
-               : dg_launch_vec<QuadraticRTarget, GlobalDenseRank1, true>(q, v, out, n, dim, m, status, st);
-  return had ? dg_launch_vec<QuadraticRTarget, GlobalDenseHadamard, false>(q, v, out, n, dim, m, status, st)
-             : dg_launch_vec<QuadraticRTarget, GlobalDenseRank1, false>(q, v, out, n, dim, m, status, st);
+    return hadamard ? dg_launch_vec<GlobalDenseHadamard, true>(a) : dg_launch_vec<GlobalDenseRank1, true>(a);
+  return hadamard ? dg_launch_vec<GlobalDenseHadamard, false>(a) : dg_launch_vec<GlobalDenseRank1, false>(a);
 }
 
 }  // namespace mb200

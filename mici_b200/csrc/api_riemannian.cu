@@ -5,32 +5,39 @@
 
 namespace mb200 {
 
-template <class Target, template <class> class MetricT>
-static int launch_implicit(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                           const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
-                           const ModelArgs& m, double fp_tol, double fp_div, int fp_max,
-                           double rev_tol, double* h_out, int32_t* status, int32_t* n_done,
-                           int32_t* fp_iters, cudaStream_t st, int midpoint, int fp_solver) {
-  auto kern = implicit_leapfrog_kernel<Target, MetricT>;
-  int n_mats = MetricT<Target>::N_MATS;
-  // SoftAbs: a third matrix enables warm-started eigensolves; use it when two CTAs still fit
-  if (MetricT<Target>::SOFTABS && rm_smem_doubles(dim, 3) * sizeof(double) <= 113 * 1024) n_mats = 3;
-  if (MetricT<Target>::SOFTABS && Target::DENSE_MTP) n_mats = 3;  // the third holds Z = A U
-  constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
-  size_t smem = (compact ? rm_compact_doubles(dim, midpoint) : rm_smem_doubles(dim, n_mats)) *
-                sizeof(double);
+// What a Riemannian entry point computes (the Hamiltonian alone is a leapfrog of zero steps)
+enum class RmOp { Leapfrog, Midpoint, SampleMomentum, Velocity };
+
+// Launch plan of the three Riemannian kernels outside the global-workspace dense policy: the
+// shared-memory layout (n_mats), the per-CTA global workspace of the policies whose matrices do
+// not fit in shared memory, and the grid.  `launch(blocks, smem, margs, n_mats)` starts `kern`.
+template <class Target, template <class> class MetricT, class Kernel, class Launch>
+static int rm_launch(Kernel kern, const char* name, RmOp op, int64_t n, int dim,
+                     const ModelArgs& m, cudaStream_t st, const Launch& launch) {
+  using Metric = MetricT<Target>;
+  constexpr bool compact = rm_compact_policy<Metric>::value;
+  constexpr int ws_mats = rm_workspace_mats<Metric>::value;
+  const bool implicit = op == RmOp::Leapfrog || op == RmOp::Midpoint;
+  int n_mats = Metric::N_MATS;
+  // SoftAbs integrators: a third matrix enables warm-started eigensolves; use it when two CTAs
+  // still fit (DENSE_MTP targets always: the third holds Z = A U)
+  if (Metric::SOFTABS && implicit &&
+      (rm_smem_doubles(dim, 3) * sizeof(double) <= 113 * 1024 || Target::DENSE_MTP))
+    n_mats = 3;
+  size_t smem = (compact ? rm_compact_doubles(dim, op == RmOp::Midpoint)
+                         : rm_smem_doubles(dim, n_mats)) * sizeof(double);
   bool in_ws = false;
-  if (compact && smem > 227 * 1024)
-    return fail(MB200_ERR_UNSUPPORTED, "dim %d: per-chain vectors (%zu bytes) exceed shared memory",
-                dim, smem);
-  constexpr int ws_mats = rm_workspace_mats<MetricT<Target>>::value;
   if (smem > 227 * 1024) {
+    if (compact && implicit)
+      return fail(MB200_ERR_UNSUPPORTED,
+                  "dim %d: per-chain vectors (%zu bytes) exceed shared memory", dim, smem);
     // SoftAbs and Cholesky-factored metrics beyond shared memory: the same kernels with the
     // matrices in a per-CTA global workspace (L2-resident operands: slower, but the reference
     // has no dimension limit)
     if (ws_mats == 0)
-      return fail(MB200_ERR_UNSUPPORTED,
-                  "dim %d: per-chain metric (%zu bytes) exceeds shared memory", dim, smem);
+      return implicit ? fail(MB200_ERR_UNSUPPORTED,
+                             "dim %d: per-chain metric (%zu bytes) exceeds shared memory", dim, smem)
+                      : fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
     n_mats = RM_NMATS_IN_WORKSPACE + ws_mats;
     smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
     in_ws = true;
@@ -38,10 +45,15 @@ static int launch_implicit(const double* q_in, const double* p_in, double* q_out
   }
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, MetricT<Target>::THREADS, smem);
-  if (per_sm < 1) per_sm = 1;
-  if (in_ws && per_sm > 2) per_sm = 2;
+  // the integrators and the small CTAs of the compact policies: as many CTAs as fit (at most two
+  // per SM with the workspace); the vector kernels of the matrix policies: two per SM
+  int per_sm = 2;
+  if (implicit || compact) {
+    per_sm = 1;
+    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, Metric::THREADS, smem);
+    if (per_sm < 1) per_sm = 1;
+    if (in_ws && per_sm > 2) per_sm = 2;
+  }
   int64_t blocks = (int64_t)num_sms() * per_sm;
   if (blocks > n) blocks = n;
   ModelArgs margs = m;
@@ -52,273 +64,186 @@ static int launch_implicit(const double* q_in, const double* p_in, double* q_out
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
-  kern<<<(unsigned)blocks, MetricT<Target>::THREADS, smem, st>>>(
-      q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, margs, fp_tol, fp_div, fp_max, rev_tol,
-      h_out, status, n_done, fp_iters, n_mats, midpoint, fp_solver);
-  return check_launch("implicit_leapfrog_kernel");
+  launch((unsigned)blocks, smem, margs, n_mats);
+  return check_launch(name);
 }
 
-// Dense metrics whose factor does not fit in shared memory (and every Hadamard metric) run through
-// the global-workspace policy (api_dense.cu); the rank-1 metric keeps its Sherman-Morrison form
-// as an OPTIONAL policy (rmetric_params[2] != 0) and for targets the dense policy is not
-// compiled for.
-static bool wants_global_dense(const ModelArgs& m, int dim) {
-  if (m.rmetric_id == MB200_RMETRIC_HADAMARD) return true;
-  if (m.rmetric_id != MB200_RMETRIC_RANK1) return false;
-  const bool fits = rm_smem_doubles(dim, 1) * sizeof(double) <= 227 * 1024;
-  return !fits && m.mp[2] == 0.0 && m.target_id == MB200_TARGET_QUADRATIC &&
-         dense_global_supported(dim);
-}
-
-static bool is_compact_rmetric(int id) {
-  return id == MB200_RMETRIC_DIAG_QUADRATIC || id == MB200_RMETRIC_DIAG_FUNNEL_FISHER ||
-         id == MB200_RMETRIC_SCALAR_QUADRATIC;
-}
-
-// Target / metric pairs of the O(D) metrics.  `L` is one of the launch functors below: its
-// `run<Target, MetricT>()` launches the entry point's kernel for that pair.
-template <class L>
-static int compact_dispatch(const ModelArgs& m, int dim, const L& l) {
-  if (m.rmetric_id != MB200_RMETRIC_DIAG_FUNNEL_FISHER && !(m.mp[0] > 0.0 && m.mp[1] >= 0.0))
-    return fail(MB200_ERR_INVALID_ARG, "metric parameters need a > 0 and b >= 0");
-  if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
-    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
-  if (m.target_id == MB200_TARGET_QUADRATIC && !m.taux)
-    return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
-  if (m.rmetric_id == MB200_RMETRIC_DIAG_FUNNEL_FISHER) {
-    if (m.target_id != MB200_TARGET_NEAL_FUNNEL)
-      return fail(MB200_ERR_UNSUPPORTED, "the funnel Fisher metric needs the funnel target (got %d)",
-                  m.target_id);
-    return l.template run<FunnelRTarget, FunnelFisherMetric>();
-  }
-  const bool diag = m.rmetric_id == MB200_RMETRIC_DIAG_QUADRATIC;
-  switch (m.target_id) {
-    case MB200_TARGET_STD_GAUSSIAN:
-      return diag ? l.template run<StdGaussianRTarget, QuadraticDiagonalMetric>()
-                  : l.template run<StdGaussianRTarget, ScalarMetric>();
-    case MB200_TARGET_BANANA:
-      return diag ? l.template run<BananaRTarget, QuadraticDiagonalMetric>()
-                  : l.template run<BananaRTarget, ScalarMetric>();
-    case MB200_TARGET_NEAL_FUNNEL:
-      return diag ? l.template run<FunnelRTarget, QuadraticDiagonalMetric>()
-                  : l.template run<FunnelRTarget, ScalarMetric>();
-    case MB200_TARGET_QUADRATIC:
-      return diag ? l.template run<QuadraticRTarget, QuadraticDiagonalMetric>()
-                  : l.template run<QuadraticRTarget, ScalarMetric>();
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d not available with diagonal / scalar metrics",
-                  m.target_id);
-  }
-}
-
-// Target / metric pairs of the Cholesky-factored metric (same targets and argument checks as
-// compact_dispatch); `L` as there
-template <class L>
-static int chol_dispatch(const ModelArgs& m, int dim, const L& l) {
-  if (!m.maux)
-    return fail(MB200_ERR_INVALID_ARG, "Cholesky-factored metric needs its base factor (rmetric_aux)");
-  if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
-    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
-  if (m.target_id == MB200_TARGET_QUADRATIC && !m.taux)
-    return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
-  switch (m.target_id) {
-    case MB200_TARGET_STD_GAUSSIAN: return l.template run<StdGaussianRTarget, QuadraticCholeskyMetric>();
-    case MB200_TARGET_BANANA: return l.template run<BananaRTarget, QuadraticCholeskyMetric>();
-    case MB200_TARGET_NEAL_FUNNEL: return l.template run<FunnelRTarget, QuadraticCholeskyMetric>();
-    case MB200_TARGET_QUADRATIC: return l.template run<QuadraticRTarget, QuadraticCholeskyMetric>();
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d not available with a Cholesky-factored metric",
-                  m.target_id);
-  }
-}
-
+// Launch functors of the operations: `run<Target, MetricT>()` starts the operation's kernel for
+// that pair, `global(hadamard)` its global-workspace dense form (api_dense.cu)
+template <RmOp OP>
 struct ImplicitLaunch {
-  const double *q_in, *p_in;
-  double *q_out, *p_out;
-  const int32_t* dir;
-  int64_t n;
-  int dim;
-  double eps;
-  int n_steps;
-  const ModelArgs& m;
-  double fp_tol, fp_div;
-  int fp_max;
-  double rev_tol;
-  double* h_out;
-  int32_t *status, *n_done, *fp_iters;
-  cudaStream_t st;
-  int midpoint, fp_solver;
+  static constexpr RmOp op = OP;
+  const ImplicitArgs& a;
   template <class Target, template <class> class MetricT>
   int run() const {
-    return launch_implicit<Target, MetricT>(q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, m,
-                                            fp_tol, fp_div, fp_max, rev_tol, h_out, status, n_done,
-                                            fp_iters, st, midpoint, fp_solver);
+    auto kern = implicit_leapfrog_kernel<Target, MetricT>;
+    return rm_launch<Target, MetricT>(
+        kern, "implicit_leapfrog_kernel", OP, a.n, a.dim, a.m, a.st,
+        [&](unsigned blocks, size_t smem, const ModelArgs& margs, int n_mats) {
+          kern<<<blocks, MetricT<Target>::THREADS, smem, a.st>>>(
+              a.q_in, a.p_in, a.q_out, a.p_out, a.dir, a.n, a.dim, a.eps, a.n_steps, margs,
+              a.fp_tol, a.fp_div, a.fp_max, a.rev_tol, a.h_out, a.status, a.n_done, a.fp_iters,
+              n_mats, (int)(OP == RmOp::Midpoint), a.fp_solver);
+        });
+  }
+  int global(bool hadamard) const { return dense_global_implicit(a, hadamard); }
+};
+
+template <RmOp OP>
+struct VectorLaunch {
+  static constexpr RmOp op = OP;
+  static constexpr bool velocity = OP == RmOp::Velocity;
+  const VectorArgs& a;
+  template <class Target, template <class> class MetricT>
+  int run() const {
+    auto kern = riemannian_vector_kernel<Target, MetricT, velocity>();
+    return rm_launch<Target, MetricT>(
+        kern, velocity ? "riemannian_velocity_kernel" : "riemannian_sample_momentum_kernel", OP,
+        a.n, a.dim, a.m, a.st, [&](unsigned blocks, size_t smem, const ModelArgs& margs, int n_mats) {
+          kern<<<blocks, MetricT<Target>::THREADS, smem, a.st>>>(a.q, a.v, a.out, a.n, a.dim,
+                                                                 margs, a.status, n_mats);
+        });
+  }
+  int global(bool hadamard) const { return dense_global_vector(a, velocity, hadamard); }
+};
+
+// The caller-provided workspace an implicit leapfrog of this model takes (the global-workspace
+// dense policy only); launches nothing
+struct WorkspaceQuery {
+  static constexpr RmOp op = RmOp::Leapfrog;
+  int64_t n;
+  int dim;
+  int64_t* bytes;
+  template <class Target, template <class> class MetricT>
+  int run() const { return 0; }
+  int global(bool) const {
+    *bytes = dense_global_workspace_bytes(n, dim);
+    return 0;
   }
 };
 
-static int implicit_dispatch(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                             const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
-                             const ModelArgs& m, double fp_tol, double fp_div, int fp_max,
-                             double rev_tol, double* h_out, int32_t* status, int32_t* n_done,
-                             int32_t* fp_iters, cudaStream_t st, int midpoint = 0,
-                             int fp_solver = 0, void* ws = nullptr, int64_t ws_bytes = 0) {
-  if (fp_solver != MB200_FP_SOLVER_DIRECT && fp_solver != MB200_FP_SOLVER_STEFFENSEN)
-    return fail(MB200_ERR_INVALID_ARG, "unknown fixed-point solver %d", fp_solver);
-  const DeviceScope device_scope(q_in);
-  if (wants_global_dense(m, dim))
-    return dense_global_implicit(q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, m, fp_tol,
-                                 fp_div, fp_max, rev_tol, h_out, status, n_done, fp_iters, st,
-                                 midpoint, fp_solver, ws, ws_bytes);
-#define MB200_ARGS                                                                           \
-  q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, m, fp_tol, fp_div, fp_max, rev_tol,   \
-      h_out, status, n_done, fp_iters, st, midpoint, fp_solver
+// `l` on the targets a metric policy is compiled for: std-Gaussian, banana, quadratic and (FUNNEL)
+// Neal's funnel; `metric` completes the error of any other target
+template <template <class> class MetricT, bool FUNNEL, class L>
+static int run_on_target(int target_id, const L& l, const char* metric) {
+  switch (target_id) {
+    case MB200_TARGET_STD_GAUSSIAN: return l.template run<StdGaussianRTarget, MetricT>();
+    case MB200_TARGET_BANANA: return l.template run<BananaRTarget, MetricT>();
+    case MB200_TARGET_QUADRATIC: return l.template run<QuadraticRTarget, MetricT>();
+    case MB200_TARGET_NEAL_FUNNEL:
+      if constexpr (FUNNEL) return l.template run<FunnelRTarget, MetricT>();
+  }
+  return fail(MB200_ERR_UNSUPPORTED, "target %d not available %s", target_id, metric);
+}
+
+// Which kernel serves a Riemannian model, for every operation L::op: checks the model (the same
+// checks whatever the operation), picks the metric policy and the target, and hands them to `l`.
+// An operation's exclusions sit next to the route they restrict.
+template <class L>
+static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
+  constexpr RmOp op = L::op;
+  const int t = m.target_id;
+  // one per-chain D x D matrix (the rank-1 metric's Cholesky factor) fits in shared memory
+  const bool fits = rm_smem_doubles(dim, 1) * sizeof(double) <= 227 * 1024;
+
+  // Global-workspace dense policy: every Hadamard metric, and the rank-1 metric whose factor does
+  // not fit in shared memory on the quadratic target, unless the Sherman-Morrison form is forced
+  // (rmetric_params[2] != 0)
+  if (m.rmetric_id == MB200_RMETRIC_HADAMARD ||
+      (m.rmetric_id == MB200_RMETRIC_RANK1 && !fits && m.mp[2] == 0.0 &&
+       t == MB200_TARGET_QUADRATIC && dense_global_supported(dim))) {
+    if (op == RmOp::Midpoint)
+      return fail(MB200_ERR_UNSUPPORTED,
+                  "implicit midpoint is not available for the global-workspace dense metric");
+    if (!dense_global_supported(dim))
+      return fail(MB200_ERR_UNSUPPORTED, "dim %d: panel buffers exceed shared memory", dim);
+    if (!m.maux) return fail(MB200_ERR_INVALID_ARG, "dense metric needs its matrices (rmetric_aux)");
+    if (t != MB200_TARGET_QUADRATIC)
+      return fail(MB200_ERR_UNSUPPORTED,
+                  "target %d not compiled for the global-workspace dense metric", t);
+    if (!m.taux) return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
+    return l.global(m.rmetric_id == MB200_RMETRIC_HADAMARD);
+  }
+
   if (m.rmetric_id == MB200_RMETRIC_SOFTABS) {
     if (!(m.mp[0] > 0.0)) return fail(MB200_ERR_INVALID_ARG, "softabs_coeff must be positive");
-    switch (m.target_id) {
-      case MB200_TARGET_BANANA:
-        if (dim & 1) return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
-        return launch_implicit<BananaRTarget, SoftAbsMetric>(MB200_ARGS);
-      case MB200_TARGET_QUARTIC:
-        if (!m.taux) return fail(MB200_ERR_INVALID_ARG, "quartic target needs its directions");
-        if (midpoint)
-          return fail(MB200_ERR_UNSUPPORTED, "implicit midpoint: quartic target not available");
-        return launch_implicit<QuarticRTarget, SoftAbsMetric>(MB200_ARGS);
-      default:
-        return fail(MB200_ERR_UNSUPPORTED, "target %d has no device Hessian / MTP (SoftAbs metric)",
-                    m.target_id);
+    if (t == MB200_TARGET_BANANA) {
+      if (dim & 1) return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
+      return l.template run<BananaRTarget, SoftAbsMetric>();
     }
-  }
-  if (m.rmetric_id == MB200_RMETRIC_RANK1) {
-    if (!m.maux) return fail(MB200_ERR_INVALID_ARG, "rank-1 metric needs its base matrix (rmetric_aux)");
-    if (m.target_id == MB200_TARGET_QUADRATIC && !m.taux)
-      return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
-    if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
-      return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
-    // per-chain Cholesky factor in shared memory when it fits (or when forced), else the
-    // Sherman-Morrison form that never materialises M(q); mp[2] != 0 forces the latter
-    // (dimensions beyond shared memory reach this point only with the Sherman-Morrison policy
-    // forced or for targets the global-workspace dense policy is not compiled for)
-    const bool fits = rm_smem_doubles(dim, 1) * sizeof(double) <= 227 * 1024;
-    const bool woodbury = !fits || m.mp[2] != 0.0;
-    switch (m.target_id) {
-      case MB200_TARGET_QUADRATIC:
-        return woodbury ? launch_implicit<QuadraticRTarget, Rank1WoodburyMetric>(MB200_ARGS)
-                        : launch_implicit<QuadraticRTarget, Rank1DenseMetric>(MB200_ARGS);
-      case MB200_TARGET_STD_GAUSSIAN:
-        return woodbury ? launch_implicit<StdGaussianRTarget, Rank1WoodburyMetric>(MB200_ARGS)
-                        : launch_implicit<StdGaussianRTarget, Rank1DenseMetric>(MB200_ARGS);
-      case MB200_TARGET_BANANA:
-        return woodbury ? launch_implicit<BananaRTarget, Rank1WoodburyMetric>(MB200_ARGS)
-                        : launch_implicit<BananaRTarget, Rank1DenseMetric>(MB200_ARGS);
-      default:
-        return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Riemannian systems", m.target_id);
+    if (t == MB200_TARGET_QUARTIC) {
+      if (!m.taux) return fail(MB200_ERR_INVALID_ARG, "quartic target needs its directions");
+      if (op == RmOp::Midpoint)
+        return fail(MB200_ERR_UNSUPPORTED, "implicit midpoint: quartic target not available");
+      return l.template run<QuarticRTarget, SoftAbsMetric>();
     }
+    return fail(MB200_ERR_UNSUPPORTED, "target %d has no device Hessian / MTP (SoftAbs metric)", t);
   }
-#undef MB200_ARGS
-  if (is_compact_rmetric(m.rmetric_id))
-    return compact_dispatch(m, dim, ImplicitLaunch{q_in, p_in, q_out, p_out, dir, n, dim, eps,
-                                                   n_steps, m, fp_tol, fp_div, fp_max, rev_tol,
-                                                   h_out, status, n_done, fp_iters, st, midpoint,
-                                                   fp_solver});
-  if (m.rmetric_id == MB200_RMETRIC_CHOL_QUADRATIC)
-    return chol_dispatch(m, dim, ImplicitLaunch{q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps,
-                                                m, fp_tol, fp_div, fp_max, rev_tol, h_out, status,
-                                                n_done, fp_iters, st, midpoint, fp_solver});
-  return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
+
+  // the other metrics' own arguments, then their targets'
+  switch (m.rmetric_id) {
+    case MB200_RMETRIC_RANK1:
+      if (!m.maux)
+        return fail(MB200_ERR_INVALID_ARG, "rank-1 metric needs its base matrix (rmetric_aux)");
+      break;
+    case MB200_RMETRIC_DIAG_QUADRATIC:
+    case MB200_RMETRIC_SCALAR_QUADRATIC:
+      if (!(m.mp[0] > 0.0 && m.mp[1] >= 0.0))
+        return fail(MB200_ERR_INVALID_ARG, "metric parameters need a > 0 and b >= 0");
+      break;
+    case MB200_RMETRIC_DIAG_FUNNEL_FISHER: break;
+    case MB200_RMETRIC_CHOL_QUADRATIC:
+      if (!m.maux)
+        return fail(MB200_ERR_INVALID_ARG,
+                    "Cholesky-factored metric needs its base factor (rmetric_aux)");
+      break;
+    default: return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
+  }
+  if (t == MB200_TARGET_BANANA && (dim & 1))
+    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
+  if (t == MB200_TARGET_QUADRATIC && !m.taux)
+    return fail(MB200_ERR_INVALID_ARG, "quadratic target needs its precision matrix");
+
+  switch (m.rmetric_id) {
+    case MB200_RMETRIC_RANK1:
+      // per-chain Cholesky factor in shared memory when it fits, else the Sherman-Morrison form
+      // that never materialises M(q); rmetric_params[2] != 0 forces the latter for the integrators
+      // and the velocity (the momentum refresh needs the factor)
+      if (!fits || (m.mp[2] != 0.0 && op != RmOp::SampleMomentum)) {
+        if constexpr (op == RmOp::SampleMomentum)
+          return fail(MB200_ERR_UNSUPPORTED,
+                      "dim %d: the Cholesky factor of M(q) does not fit in shared memory", dim);
+        else
+          return run_on_target<Rank1WoodburyMetric, false>(t, l, "for Riemannian systems");
+      }
+      return run_on_target<Rank1DenseMetric, false>(t, l, "for Riemannian systems");
+    case MB200_RMETRIC_DIAG_FUNNEL_FISHER:
+      if (t != MB200_TARGET_NEAL_FUNNEL)
+        return fail(MB200_ERR_UNSUPPORTED,
+                    "the funnel Fisher metric needs the funnel target (got %d)", t);
+      return l.template run<FunnelRTarget, FunnelFisherMetric>();
+    case MB200_RMETRIC_DIAG_QUADRATIC:
+      return run_on_target<QuadraticDiagonalMetric, true>(t, l, "with diagonal / scalar metrics");
+    case MB200_RMETRIC_SCALAR_QUADRATIC:
+      return run_on_target<ScalarMetric, true>(t, l, "with diagonal / scalar metrics");
+    default:
+      return run_on_target<QuadraticCholeskyMetric, true>(t, l, "with a Cholesky-factored metric");
+  }
 }
 
-template <class Target, template <class> class MetricT>
-static int launch_sample_momentum(const double* q, const double* z, double* p_out, int64_t n,
-                                  int dim, const ModelArgs& m, int32_t* status, cudaStream_t st) {
-  auto kern = riemannian_sample_momentum_kernel<Target, MetricT>;
-  int n_mats = MetricT<Target>::N_MATS;
-  constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
-  size_t smem = (compact ? rm_compact_doubles(dim, 0) : rm_smem_doubles(dim, n_mats)) * sizeof(double);
-  bool in_ws = false;
-  constexpr int ws_mats = rm_workspace_mats<MetricT<Target>>::value;
-  if (smem > 227 * 1024) {
-    if (ws_mats == 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
-    n_mats = RM_NMATS_IN_WORKSPACE + ws_mats;
-    smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
-    in_ws = true;
-    if (smem > 227 * 1024) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
-  }
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  int64_t blocks = (int64_t)num_sms() * 2;
-  if (compact) {  // small CTAs: as many as fit
-    int per_sm = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, MetricT<Target>::THREADS, smem);
-    blocks = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
-  }
-  if (blocks > n) blocks = n;
-  ModelArgs margs = m;
-  const size_t per_cta = ws_mats * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
-  DgScratch scratch(nullptr, 0, in_ws ? per_cta * blocks * sizeof(double) : 0, st);
-  if (in_ws) {
-    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "metric workspace allocation failed");
-    margs.workspace = scratch.ptr;
-    margs.ws_stride = per_cta;
-  }
-  kern<<<(unsigned)blocks, MetricT<Target>::THREADS, smem, st>>>(q, z, p_out, n, dim, margs, status,
-                                                                  n_mats);
-  return check_launch("riemannian_sample_momentum_kernel");
+template <RmOp OP>
+static int implicit_dispatch(const ImplicitArgs& a) {
+  if (a.fp_solver != MB200_FP_SOLVER_DIRECT && a.fp_solver != MB200_FP_SOLVER_STEFFENSEN)
+    return fail(MB200_ERR_INVALID_ARG, "unknown fixed-point solver %d", a.fp_solver);
+  const DeviceScope device_scope(a.q_in);
+  return rm_dispatch(a.m, a.dim, ImplicitLaunch<OP>{a});
 }
 
-template <class Target, template <class> class MetricT>
-static int launch_velocity(const double* q, const double* p, double* vel, int64_t n, int dim,
-                           const ModelArgs& m, int32_t* status, cudaStream_t st) {
-  auto kern = riemannian_velocity_kernel<Target, MetricT>;
-  int n_mats = MetricT<Target>::N_MATS;
-  constexpr bool compact = rm_compact_policy<MetricT<Target>>::value;
-  size_t smem = (compact ? rm_compact_doubles(dim, 0) : rm_smem_doubles(dim, n_mats)) * sizeof(double);
-  bool in_ws = false;
-  constexpr int ws_mats = rm_workspace_mats<MetricT<Target>>::value;
-  if (smem > 227 * 1024) {
-    if (ws_mats == 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
-    n_mats = RM_NMATS_IN_WORKSPACE + ws_mats;
-    smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
-    in_ws = true;
-    if (smem > 227 * 1024) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
-  }
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  int64_t blocks = (int64_t)num_sms() * 2;
-  if (compact) {  // small CTAs: as many as fit
-    int per_sm = 1;
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, MetricT<Target>::THREADS, smem);
-    blocks = (int64_t)num_sms() * (per_sm > 1 ? per_sm : 1);
-  }
-  if (blocks > n) blocks = n;
-  ModelArgs margs = m;
-  const size_t per_cta = ws_mats * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
-  DgScratch scratch(nullptr, 0, in_ws ? per_cta * blocks * sizeof(double) : 0, st);
-  if (in_ws) {
-    if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "metric workspace allocation failed");
-    margs.workspace = scratch.ptr;
-    margs.ws_stride = per_cta;
-  }
-  kern<<<(unsigned)blocks, MetricT<Target>::THREADS, smem, st>>>(q, p, vel, n, dim, margs, status,
-                                                                  n_mats);
-  return check_launch("riemannian_velocity_kernel");
+template <RmOp OP>
+static int vector_dispatch(const VectorArgs& a) {
+  const DeviceScope device_scope(a.q);
+  return rm_dispatch(a.m, a.dim, VectorLaunch<OP>{a});
 }
-
-// sqrt(M(q)) v (velocity = false) or M(q)^-1 v (velocity = true) for the compact metrics
-struct VectorLaunch {
-  const double *q, *v;
-  double* out;
-  int64_t n;
-  int dim;
-  const ModelArgs& m;
-  int32_t* status;
-  cudaStream_t st;
-  bool velocity;
-  template <class Target, template <class> class MetricT>
-  int run() const {
-    return velocity ? launch_velocity<Target, MetricT>(q, v, out, n, dim, m, status, st)
-                    : launch_sample_momentum<Target, MetricT>(q, v, out, n, dim, m, status, st);
-  }
-};
 
 }  // namespace mb200
 
@@ -339,11 +264,11 @@ int mb200_implicit_leapfrog_riemannian(
   if (n_chains < 0 || dim < 1 || n_steps < 0 || fp_max_iters < 0)
     return fail(MB200_ERR_INVALID_ARG, "bad sizes");
   if (n_chains == 0) return 0;
-  return implicit_dispatch(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                           n_steps, to_args(model, step_sizes, n_steps_per_chain),
-                           fp_convergence_tol, fp_divergence_tol, fp_max_iters, reverse_check_tol,
-                           h_out, status, n_done, fp_iters, (cudaStream_t)stream, 0, fp_solver,
-                           workspace, workspace_bytes);
+  return implicit_dispatch<RmOp::Leapfrog>(ImplicitArgs{
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps,
+      to_args(model, step_sizes, n_steps_per_chain), fp_convergence_tol, fp_divergence_tol,
+      fp_max_iters, reverse_check_tol, h_out, status, n_done, fp_iters, fp_solver, workspace,
+      workspace_bytes, (cudaStream_t)stream});
 }
 
 // Per-chain buffers live in shared memory except for the global-workspace dense metric policy
@@ -351,8 +276,9 @@ int mb200_implicit_leapfrog_riemannian(
 // library then takes the scratch from the stream-ordered allocator for the duration of the call.
 int64_t mb200_implicit_workspace_bytes(int64_t n_chains, int32_t dim, const mb200_model* model) {
   if (!model || n_chains <= 0 || dim < 1) return 0;
-  const ModelArgs m = to_args(model);
-  return wants_global_dense(m, dim) ? dense_global_workspace_bytes(n_chains, dim) : 0;
+  int64_t bytes = 0;
+  rm_dispatch(to_args(model), dim, WorkspaceQuery{n_chains, dim, &bytes});
+  return bytes;
 }
 
 int mb200_hamiltonian_riemannian(const double* pos, const double* mom, int64_t n_chains,
@@ -364,10 +290,10 @@ int mb200_hamiltonian_riemannian(const double* pos, const double* mom, int64_t n
   if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
   if (n_chains == 0) return 0;
   // zero steps: state written back unchanged in place, h evaluated
-  return implicit_dispatch(pos, mom, const_cast<double*>(pos), const_cast<double*>(mom), nullptr,
-                           n_chains, dim, 0.0, 0, to_args(model), 1e-9, 1e10, 100, 2e-8, h_out,
-                           status, nullptr, nullptr, (cudaStream_t)stream, 0, 0, workspace,
-                           workspace_bytes);
+  return implicit_dispatch<RmOp::Leapfrog>(ImplicitArgs{
+      pos, mom, const_cast<double*>(pos), const_cast<double*>(mom), nullptr, n_chains, dim, 0.0, 0,
+      to_args(model), 1e-9, 1e10, 100, 2e-8, h_out, status, nullptr, nullptr,
+      MB200_FP_SOLVER_DIRECT, workspace, workspace_bytes, (cudaStream_t)stream});
 }
 
 int mb200_selftest_fixed_point(int32_t func_id, int32_t fp_solver, const double* x0,
@@ -418,11 +344,11 @@ int mb200_implicit_midpoint_riemannian(
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_chains < 0 || dim < 1 || n_steps < 0 || fp_max_iters < 0)
     return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  return implicit_dispatch(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                           n_steps, to_args(model, step_sizes, n_steps_per_chain),
-                           fp_convergence_tol, fp_divergence_tol,
-                           fp_max_iters, reverse_check_tol, h_out, status, n_done, fp_iters,
-                           (cudaStream_t)stream, 1, fp_solver);
+  return implicit_dispatch<RmOp::Midpoint>(ImplicitArgs{
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps,
+      to_args(model, step_sizes, n_steps_per_chain), fp_convergence_tol, fp_divergence_tol,
+      fp_max_iters, reverse_check_tol, h_out, status, n_done, fp_iters, fp_solver, nullptr, 0,
+      (cudaStream_t)stream});
 }
 
 int mb200_sample_momentum_riemannian(const double* pos, const double* normals, double* mom_out,
@@ -431,37 +357,8 @@ int mb200_sample_momentum_riemannian(const double* pos, const double* normals, d
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos || !normals || !mom_out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  const DeviceScope device_scope(pos);
-  const ModelArgs m = to_args(model);
-  cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS pos, normals, mom_out, n_chains, dim, m, status, st
-  if (wants_global_dense(m, dim))
-    return dense_global_vector(pos, normals, mom_out, n_chains, dim, m, status, st, 0);
-  if (m.rmetric_id == MB200_RMETRIC_SOFTABS) {
-    if (m.target_id == MB200_TARGET_BANANA) return launch_sample_momentum<BananaRTarget, SoftAbsMetric>(MB200_ARGS);
-    if (m.target_id == MB200_TARGET_QUARTIC) return launch_sample_momentum<QuarticRTarget, SoftAbsMetric>(MB200_ARGS);
-    return fail(MB200_ERR_UNSUPPORTED, "target %d has no device Hessian", m.target_id);
-  }
-  if (m.rmetric_id == MB200_RMETRIC_RANK1) {
-    if (!m.maux) return fail(MB200_ERR_INVALID_ARG, "rank-1 metric needs its base matrix");
-    if (rm_smem_doubles(dim, 1) * sizeof(double) > 227 * 1024)
-      return fail(MB200_ERR_UNSUPPORTED,
-                  "dim %d: the Cholesky factor of M(q) does not fit in shared memory", dim);
-    switch (m.target_id) {
-      case MB200_TARGET_QUADRATIC: return launch_sample_momentum<QuadraticRTarget, Rank1DenseMetric>(MB200_ARGS);
-      case MB200_TARGET_STD_GAUSSIAN: return launch_sample_momentum<StdGaussianRTarget, Rank1DenseMetric>(MB200_ARGS);
-      case MB200_TARGET_BANANA: return launch_sample_momentum<BananaRTarget, Rank1DenseMetric>(MB200_ARGS);
-      default: return fail(MB200_ERR_UNSUPPORTED, "target %d not available", m.target_id);
-    }
-  }
-#undef MB200_ARGS
-  if (is_compact_rmetric(m.rmetric_id))
-    return compact_dispatch(m, dim, VectorLaunch{pos, normals, mom_out, n_chains, dim, m, status,
-                                                 st, false});
-  if (m.rmetric_id == MB200_RMETRIC_CHOL_QUADRATIC)
-    return chol_dispatch(m, dim, VectorLaunch{pos, normals, mom_out, n_chains, dim, m, status, st,
-                                              false});
-  return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
+  return vector_dispatch<RmOp::SampleMomentum>(
+      VectorArgs{pos, normals, mom_out, n_chains, dim, to_args(model), status, (cudaStream_t)stream});
 }
 
 int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_out,
@@ -470,41 +367,8 @@ int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_o
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos || !mom || !vel_out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  const DeviceScope device_scope(pos);
-  const ModelArgs m = to_args(model);
-  cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS pos, mom, vel_out, n_chains, dim, m, status, st
-  if (wants_global_dense(m, dim))
-    return dense_global_vector(pos, mom, vel_out, n_chains, dim, m, status, st, 1);
-  if (m.rmetric_id == MB200_RMETRIC_SOFTABS) {
-    if (m.target_id == MB200_TARGET_BANANA) return launch_velocity<BananaRTarget, SoftAbsMetric>(MB200_ARGS);
-    if (m.target_id == MB200_TARGET_QUARTIC) return launch_velocity<QuarticRTarget, SoftAbsMetric>(MB200_ARGS);
-    return fail(MB200_ERR_UNSUPPORTED, "target %d has no device Hessian", m.target_id);
-  }
-  if (m.rmetric_id == MB200_RMETRIC_RANK1) {
-    if (!m.maux) return fail(MB200_ERR_INVALID_ARG, "rank-1 metric needs its base matrix");
-    const bool fits = rm_smem_doubles(dim, 1) * sizeof(double) <= 227 * 1024;
-    const bool woodbury = !fits || m.mp[2] != 0.0;
-    switch (m.target_id) {
-      case MB200_TARGET_QUADRATIC:
-        return woodbury ? launch_velocity<QuadraticRTarget, Rank1WoodburyMetric>(MB200_ARGS)
-                        : launch_velocity<QuadraticRTarget, Rank1DenseMetric>(MB200_ARGS);
-      case MB200_TARGET_STD_GAUSSIAN:
-        return woodbury ? launch_velocity<StdGaussianRTarget, Rank1WoodburyMetric>(MB200_ARGS)
-                        : launch_velocity<StdGaussianRTarget, Rank1DenseMetric>(MB200_ARGS);
-      case MB200_TARGET_BANANA:
-        return woodbury ? launch_velocity<BananaRTarget, Rank1WoodburyMetric>(MB200_ARGS)
-                        : launch_velocity<BananaRTarget, Rank1DenseMetric>(MB200_ARGS);
-      default: return fail(MB200_ERR_UNSUPPORTED, "target %d not available", m.target_id);
-    }
-  }
-#undef MB200_ARGS
-  if (is_compact_rmetric(m.rmetric_id))
-    return compact_dispatch(m, dim, VectorLaunch{pos, mom, vel_out, n_chains, dim, m, status, st,
-                                                 true});
-  if (m.rmetric_id == MB200_RMETRIC_CHOL_QUADRATIC)
-    return chol_dispatch(m, dim, VectorLaunch{pos, mom, vel_out, n_chains, dim, m, status, st, true});
-  return fail(MB200_ERR_INVALID_ARG, "unknown rmetric_id %d", m.rmetric_id);
+  return vector_dispatch<RmOp::Velocity>(
+      VectorArgs{pos, mom, vel_out, n_chains, dim, to_args(model), status, (cudaStream_t)stream});
 }
 
 }  // extern "C"

@@ -2190,4 +2190,14 @@ __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN
   }
 }
 
+// The velocity kernel (VELOCITY) or the momentum-refresh kernel of a target / metric pair; only
+// the one asked for is instantiated
+template <class Target, template <class> class MetricT, bool VELOCITY>
+inline auto riemannian_vector_kernel() {
+  if constexpr (VELOCITY)
+    return riemannian_velocity_kernel<Target, MetricT>;
+  else
+    return riemannian_sample_momentum_kernel<Target, MetricT>;
+}
+
 }  // namespace mb200
