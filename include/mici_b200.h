@@ -36,7 +36,14 @@
 #ifndef MICI_B200_H
 #define MICI_B200_H
 
+#ifndef __CUDACC_RTC__
 #include <stdint.h>
+#else /* NVRTC (user targets, mici_b200/jit.py): no system headers; LP64 integer types */
+typedef int int32_t;
+typedef unsigned int uint32_t;
+typedef long int64_t;
+typedef unsigned long uint64_t;
+#endif
 
 #ifdef __cplusplus
 extern "C" {
@@ -69,6 +76,9 @@ extern "C" {
 #define MB200_TARGET_SPHERE 5       /* tilted density on unit sphere    params: -            */
 #define MB200_TARGET_MULTI_SPHERE 6 /* n_constr unit spheres on consecutive blocks  params: n_constr (2, 4 or 8) */
 #define MB200_TARGET_QUARTIC 7      /* l = |q|^2/2 + gamma/4 sum_m (a_m.q)^4   params: gamma; aux: A [dim*dim] (dense Hessian; SoftAbs systems) */
+/* a user-written target compiled at run time (mb200_user_target_load); only the *_user entry
+ * points accept it, every registry entry point rejects it as an unknown target */
+#define MB200_TARGET_USER 64
 /* constrained targets: target_params[MB200_MAX_PARAMS - 1] != 0 means the density is given with
  * respect to the Lebesgue measure (dens_wrt_hausdorff=False, systems.py:853-861): h1 and dh1_dpos
  * carry log det gram / 2 and its gradient (systems.py:1024-1031) */
@@ -188,6 +198,43 @@ int mb200_euclidean_eval(const double* pos, const double* mom, int64_t n_chains,
                          int32_t metric_kind, const double* metric_inv, const mb200_model* model,
                          double* nld_out, double* grad_out, double* vel_out, double* kin_out,
                          void* stream);
+
+/*
+ * User-written targets (mici_b200/csrc/user_target.cuh): a model's two device functions compiled
+ * at run time, by NVRTC, together with the general-dimension Euclidean kernels.
+ *  - mb200_user_target_load: loads a CUBIN `image` of `image_bytes` (cudaLibraryLoadData; the
+ *    kernels are device-independent) and looks up its `n_names` = 10 kernels by their lowered
+ *    names, in this order: leapfrog_generic_kernel<UserTarget, KP, CPW, false> for (KP, CPW) =
+ *    (1, 4), (2, 4), (4, 2), (8, 1), (16, 1), then euclidean_eval_kernel<UserTarget, KP> for
+ *    KP = 1, 2, 4, 8, 16.  *handle receives the loaded target.
+ *  - mb200_user_target_unload: releases a handle.
+ *  - mb200_leapfrog_euclidean_user, mb200_hamiltonian_euclidean_user, mb200_euclidean_eval_user:
+ *    the same contracts as mb200_leapfrog_euclidean (always on the general-dimension kernel),
+ *    mb200_hamiltonian_euclidean and mb200_euclidean_eval, for model->target_id ==
+ *    MB200_TARGET_USER and the loaded `user_target`; dim <= 1024.
+ * The library does not link NVRTC: compiling is the caller's job (mici_b200/jit.py).
+ */
+int mb200_user_target_load(const void* image, int64_t image_bytes, const char* const* names,
+                           int32_t n_names, void** handle);
+int mb200_user_target_unload(void* handle);
+int mb200_leapfrog_euclidean_user(const double* pos_in, const double* mom_in, double* pos_out,
+                                  double* mom_out, const int32_t* dir, int64_t n_chains,
+                                  int32_t dim, double step_size, const double* step_sizes,
+                                  int32_t n_steps, const int32_t* n_steps_per_chain,
+                                  int32_t n_flows, const double* coefficients,
+                                  int32_t initial_h1_flow_step, int32_t metric_kind,
+                                  const double* metric_inv, const mb200_model* model,
+                                  double* h_out, int32_t* status, int32_t* n_done, void* stream,
+                                  const void* user_target);
+int mb200_hamiltonian_euclidean_user(const double* pos, const double* mom, int64_t n_chains,
+                                     int32_t dim, int32_t metric_kind, const double* metric_inv,
+                                     const mb200_model* model, double* h_out, void* stream,
+                                     const void* user_target);
+int mb200_euclidean_eval_user(const double* pos, const double* mom, int64_t n_chains, int32_t dim,
+                              int32_t metric_kind, const double* metric_inv,
+                              const mb200_model* model, double* nld_out, double* grad_out,
+                              double* vel_out, double* kin_out, void* stream,
+                              const void* user_target);
 
 /*
  * n_steps constrained (RATTLE / geodesic) leapfrog steps with Newton projection.

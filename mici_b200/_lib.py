@@ -71,6 +71,12 @@ SIGNATURES = {
     "mb200_leapfrog_euclidean_generic": (ctypes.c_int, _LEAPFROG_EUCLIDEAN_ARGS),
     "mb200_hamiltonian_euclidean": (ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P]),
     "mb200_euclidean_eval": (ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P, _P, _P, _P]),
+    "mb200_user_target_load": (ctypes.c_int, [ctypes.c_char_p, _I64, _P, _I32, _P]),
+    "mb200_user_target_unload": (ctypes.c_int, [_P]),
+    "mb200_leapfrog_euclidean_user": (ctypes.c_int, _LEAPFROG_EUCLIDEAN_ARGS + [_P]),
+    "mb200_hamiltonian_euclidean_user": (ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P, _P]),
+    "mb200_euclidean_eval_user": (
+        ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P, _P, _P, _P, _P]),
     "mb200_constrained_leapfrog_euclidean": (
         ctypes.c_int,
         [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _MP]

@@ -101,29 +101,61 @@ static bool is_pageable(const void* ptr) {
   return a.type == cudaMemoryTypeUnregistered;
 }
 
-template <class Target, int KP, int CPW, bool GAUSS = false>
-static int launch_generic(const double* q_in, const double* p_in, double* q_out, double* p_out,
+// One launch of the general-dimension kernel `kern` (a leapfrog_generic_kernel<Target, KP, CPW,
+// GAUSS> of the library or of a user-target image).  whole_vector: the target stages each chain's
+// position and gradient in shared memory (user_target.cuh), 2 * 64 KP doubles per warp more.
+static int launch_generic(const void* kern, int kp, int cpw, bool whole_vector,
+                          const double* q_in, const double* p_in, double* q_out, double* p_out,
                           const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
                           const FlowSchedule& sched, int metric_kind, const double* minv, const ModelArgs& m, double* h_out,
                           int32_t* status, int32_t* n_done, cudaStream_t st) {
   constexpr int WARPS = 4;
-  auto kern = leapfrog_generic_kernel<Target, KP, CPW, GAUSS>;
-  const size_t smem = (size_t)WARPS * CPW * 64 * KP * sizeof(double);
+  const size_t smem = (size_t)WARPS * (cpw + (whole_vector ? 2 : 0)) * 64 * kp * sizeof(double);
   if (smem > 48 * 1024) {
     cudaError_t e =
         cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
   }
-  const int64_t groups = (n + CPW - 1) / CPW;
+  const int64_t groups = (n + cpw - 1) / cpw;
   int64_t blocks = (groups + WARPS - 1) / WARPS;
   const int64_t cap = (int64_t)num_sms() * 16;
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
-  kern<<<(unsigned)blocks, WARPS * 32, smem, st>>>(q_in, p_in, q_out, p_out, dir, n, dim, eps,
-                                                   n_steps, sched, metric_kind, minv, m, h_out,
-                                                   status, n_done);
+  FlowSchedule sc = sched;
+  ModelArgs ma = m;
+  void* args[] = {&q_in, &p_in, &q_out, &p_out, &dir, &n, &dim, &eps, &n_steps, &sc,
+                  &metric_kind, &minv, &ma, &h_out, &status, &n_done};
+  const cudaError_t e =
+      cudaLaunchKernel(kern, dim3((unsigned)blocks), dim3(WARPS * 32), args, smem, st);
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // reported here: clear it from the runtime's error state
+    return fail(MB200_ERR_CUDA, "leapfrog_generic_kernel: %s", cudaGetErrorString(e));
+  }
   return check_launch("leapfrog_generic_kernel");
 }
+
+// (KP, CPW) of the general-dimension kernel by dimension, in the order of a user target's kernel
+// table (mb200_user_target_load)
+constexpr int N_GENERIC_LAYOUTS = 5;
+constexpr int GENERIC_KP[N_GENERIC_LAYOUTS] = {1, 2, 4, 8, 16};
+constexpr int GENERIC_CPW[N_GENERIC_LAYOUTS] = {4, 4, 2, 1, 1};
+static int generic_layout(int dim) {
+  if (dim <= 64) return 0;
+  if (dim <= 128) return 1;
+  if (dim <= 256) return 2;
+  if (dim <= 512) return 3;
+  if (dim <= 1024) return 4;
+  return -1;
+}
+
+// A loaded user-target image (mb200_user_target_load): its general-dimension leapfrog kernels
+// leapfrog_generic_kernel<UserTarget, KP, CPW, false> and evaluation kernels
+// euclidean_eval_kernel<UserTarget, KP>, one per layout of generic_layout().
+struct UserKernels {
+  cudaLibrary_t lib;
+  const void* leapfrog[N_GENERIC_LAYOUTS];
+  const void* eval[N_GENERIC_LAYOUTS];
+};
 
 template <class Target>
 static int dispatch_generic_dim(const double* q_in, const double* p_in, double* q_out,
@@ -131,19 +163,21 @@ static int dispatch_generic_dim(const double* q_in, const double* p_in, double* 
                                 int n_steps, const FlowSchedule& sched, int metric_kind, const double* minv,
                                 const ModelArgs& m, double* h_out, int32_t* status,
                                 int32_t* n_done, cudaStream_t st) {
-#define MB200_GEN(KP, CPW)                                                                      \
-  return sched.gaussian                                                                         \
-             ? launch_generic<Target, KP, CPW, true>(q_in, p_in, q_out, p_out, dir, n, dim, eps, \
-                                                     n_steps, sched, metric_kind, minv, m,      \
-                                                     h_out, status, n_done, st)                 \
-             : launch_generic<Target, KP, CPW, false>(q_in, p_in, q_out, p_out, dir, n, dim,    \
-                                                      eps, n_steps, sched, metric_kind, minv,   \
-                                                      m, h_out, status, n_done, st)
-  if (dim <= 64) MB200_GEN(1, 4);
-  if (dim <= 128) MB200_GEN(2, 4);
-  if (dim <= 256) MB200_GEN(4, 2);
-  if (dim <= 512) MB200_GEN(8, 1);
-  if (dim <= 1024) MB200_GEN(16, 1);
+#define MB200_GEN(L)                                                                          \
+  {                                                                                           \
+    constexpr int KP = GENERIC_KP[L], CPW = GENERIC_CPW[L];                                   \
+    const void* kern = sched.gaussian ? (const void*)leapfrog_generic_kernel<Target, KP, CPW, true> \
+                                      : (const void*)leapfrog_generic_kernel<Target, KP, CPW, false>; \
+    return launch_generic(kern, KP, CPW, false, q_in, p_in, q_out, p_out, dir, n, dim, eps,   \
+                          n_steps, sched, metric_kind, minv, m, h_out, status, n_done, st);   \
+  }
+  switch (generic_layout(dim)) {
+    case 0: MB200_GEN(0);
+    case 1: MB200_GEN(1);
+    case 2: MB200_GEN(2);
+    case 3: MB200_GEN(3);
+    case 4: MB200_GEN(4);
+  }
 #undef MB200_GEN
   return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported by the Euclidean leapfrog", dim);
 }
@@ -176,7 +210,8 @@ static int leapfrog_euclidean_impl(const double* q_in, const double* p_in, doubl
                                    double eps, int n_steps, const FlowSchedule& sched,
                                    int metric_kind, const double* minv, const mb200_model* model,
                                    double* h_out, int32_t* status, int32_t* n_done,
-                                   cudaStream_t st, bool allow_dmma) {
+                                   cudaStream_t st, bool allow_dmma,
+                                   const UserKernels* user = nullptr) {
   if (n == 0 && dim >= 1 && n_steps >= 0) return 0;  // empty batch: nothing to do
   if (!q_in || !p_in || !q_out || !p_out || !model)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
@@ -198,6 +233,13 @@ static int leapfrog_euclidean_impl(const double* q_in, const double* p_in, doubl
 #define MB200_ARGS                                                                         \
   q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, sched, metric_kind, minv, m, h_out, \
       status, n_done, st
+  if (user != nullptr) {
+    if (m.target_id != MB200_TARGET_USER)
+      return fail(MB200_ERR_INVALID_ARG, "user-target entry point needs target_id MB200_TARGET_USER");
+    const int l = generic_layout(dim);
+    if (l < 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported by user targets", dim);
+    return launch_generic(user->leapfrog[l], GENERIC_KP[l], GENERIC_CPW[l], true, MB200_ARGS);
+  }
   switch (m.target_id) {
     case MB200_TARGET_STD_GAUSSIAN:
       return dispatch_generic_dim<StdGaussianTarget>(MB200_ARGS);
@@ -220,7 +262,8 @@ static int leapfrog_euclidean_entry(const double* q_in, const double* p_in, doub
                                     const double* coefficients, int initial_h1_flow_step,
                                     int metric_kind, const double* minv, const mb200_model* model,
                                     double* h_out, int32_t* status, int32_t* n_done,
-                                    cudaStream_t st, bool allow_dmma) {
+                                    cudaStream_t st, bool allow_dmma,
+                                    const UserKernels* user = nullptr) {
   FlowSchedule s;
   if (const int rc = make_schedule(s, n_flows, coefficients, initial_h1_flow_step)) return rc;
   s.step_sizes = step_sizes;
@@ -229,21 +272,34 @@ static int leapfrog_euclidean_entry(const double* q_in, const double* p_in, doub
   // step sizes it scales the momentum tile by eps_c
   allow_dmma = allow_dmma && coefficients == nullptr && n_steps_pc == nullptr;
   return leapfrog_euclidean_impl(q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, s,
-                                 metric_kind, minv, model, h_out, status, n_done, st, allow_dmma);
+                                 metric_kind, minv, model, h_out, status, n_done, st, allow_dmma,
+                                 user);
 }
 
-template <class Target, int KP>
-static int launch_eval(const double* q, const double* p, int64_t n, int dim, int metric_kind,
-                       const double* minv, const ModelArgs& m, double* nld, double* grad,
-                       double* vel, double* kin, cudaStream_t st) {
+// One launch of `kern`, a euclidean_eval_kernel<Target, KP> of the library or of a user-target
+// image (whole_vector: 2 * 64 KP more doubles of shared memory per warp, as in launch_generic).
+static int launch_eval(const void* kern, int kp, bool whole_vector, const double* q,
+                       const double* p, int64_t n, int dim, int metric_kind, const double* minv,
+                       const ModelArgs& m, double* nld, double* grad, double* vel, double* kin,
+                       cudaStream_t st) {
   constexpr int WARPS = 4;
-  auto kern = euclidean_eval_kernel<Target, KP>;
-  const size_t smem = (size_t)WARPS * 64 * KP * sizeof(double);
+  const size_t smem = (size_t)WARPS * (whole_vector ? 3 : 1) * 64 * kp * sizeof(double);
+  if (smem > 48 * 1024) {
+    cudaError_t e =
+        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
+  }
   int64_t blocks = (n + WARPS - 1) / WARPS;
   const int64_t cap = (int64_t)num_sms() * 16;
   if (blocks > cap) blocks = cap;
-  kern<<<(unsigned)blocks, WARPS * 32, smem, st>>>(q, p, n, dim, metric_kind, minv, m, nld, grad,
-                                                   vel, kin);
+  ModelArgs ma = m;
+  void* args[] = {&q, &p, &n, &dim, &metric_kind, &minv, &ma, &nld, &grad, &vel, &kin};
+  const cudaError_t e =
+      cudaLaunchKernel(kern, dim3((unsigned)blocks), dim3(WARPS * 32), args, smem, st);
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // reported here: clear it from the runtime's error state
+    return fail(MB200_ERR_CUDA, "euclidean_eval_kernel: %s", cudaGetErrorString(e));
+  }
   return check_launch("euclidean_eval_kernel");
 }
 
@@ -251,15 +307,51 @@ template <class Target>
 static int dispatch_eval_dim(const double* q, const double* p, int64_t n, int dim,
                              int metric_kind, const double* minv, const ModelArgs& m, double* nld,
                              double* grad, double* vel, double* kin, cudaStream_t st) {
-#define MB200_EV(KP) \
-  return launch_eval<Target, KP>(q, p, n, dim, metric_kind, minv, m, nld, grad, vel, kin, st)
-  if (dim <= 64) MB200_EV(1);
-  if (dim <= 128) MB200_EV(2);
-  if (dim <= 256) MB200_EV(4);
-  if (dim <= 512) MB200_EV(8);
-  if (dim <= 1024) MB200_EV(16);
+#define MB200_EV(L)                                                                           \
+  return launch_eval((const void*)euclidean_eval_kernel<Target, GENERIC_KP[L]>, GENERIC_KP[L],  \
+                     false, q, p, n, dim, metric_kind, minv, m, nld, grad, vel, kin, st)
+  switch (generic_layout(dim)) {
+    case 0: MB200_EV(0);
+    case 1: MB200_EV(1);
+    case 2: MB200_EV(2);
+    case 3: MB200_EV(3);
+    case 4: MB200_EV(4);
+  }
 #undef MB200_EV
   return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported", dim);
+}
+
+// mb200_euclidean_eval and mb200_euclidean_eval_user (user != NULL)
+static int euclidean_eval_impl(const double* pos, const double* mom, int64_t n_chains, int dim,
+                               int metric_kind, const double* metric_inv,
+                               const mb200_model* model, double* nld_out, double* grad_out,
+                               double* vel_out, double* kin_out, cudaStream_t st,
+                               const UserKernels* user) {
+  if (n_chains == 0 && dim >= 1) return 0;
+  if (!pos || !mom || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
+  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
+  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
+    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
+  if (n_chains == 0) return 0;
+  const DeviceScope device_scope(pos);
+  const ModelArgs m = to_args(model);
+#define MB200_ARGS pos, mom, n_chains, dim, metric_kind, metric_inv, m, nld_out, grad_out, vel_out, kin_out, st
+  if (user != nullptr) {
+    if (m.target_id != MB200_TARGET_USER)
+      return fail(MB200_ERR_INVALID_ARG, "user-target entry point needs target_id MB200_TARGET_USER");
+    const int l = generic_layout(dim);
+    if (l < 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported by user targets", dim);
+    return launch_eval(user->eval[l], GENERIC_KP[l], true, MB200_ARGS);
+  }
+  switch (m.target_id) {
+    case MB200_TARGET_STD_GAUSSIAN: return dispatch_eval_dim<StdGaussianTarget>(MB200_ARGS);
+    case MB200_TARGET_NEAL_FUNNEL: return dispatch_eval_dim<NealFunnelTarget>(MB200_ARGS);
+    case MB200_TARGET_BANANA: return dispatch_eval_dim<BananaTarget>(MB200_ARGS);
+    default:
+      return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Euclidean eval", m.target_id);
+  }
+#undef MB200_ARGS
 }
 
 }  // namespace mb200
@@ -315,25 +407,8 @@ int mb200_euclidean_eval(const double* pos, const double* mom, int64_t n_chains,
                          int32_t metric_kind, const double* metric_inv, const mb200_model* model,
                          double* nld_out, double* grad_out, double* vel_out, double* kin_out,
                          void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos || !mom || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
-  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
-    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
-  if (n_chains == 0) return 0;
-  const DeviceScope device_scope(pos);
-  const ModelArgs m = to_args(model);
-  cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS pos, mom, n_chains, dim, metric_kind, metric_inv, m, nld_out, grad_out, vel_out, kin_out, st
-  switch (m.target_id) {
-    case MB200_TARGET_STD_GAUSSIAN: return dispatch_eval_dim<StdGaussianTarget>(MB200_ARGS);
-    case MB200_TARGET_NEAL_FUNNEL: return dispatch_eval_dim<NealFunnelTarget>(MB200_ARGS);
-    case MB200_TARGET_BANANA: return dispatch_eval_dim<BananaTarget>(MB200_ARGS);
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Euclidean eval", m.target_id);
-  }
-#undef MB200_ARGS
+  return euclidean_eval_impl(pos, mom, n_chains, dim, metric_kind, metric_inv, model, nld_out,
+                             grad_out, vel_out, kin_out, (cudaStream_t)stream, nullptr);
 }
 
 int mb200_leapfrog_gaussian_euclidean(const double* pos_in, const double* mom_in, double* pos_out,
@@ -357,6 +432,84 @@ int mb200_leapfrog_gaussian_euclidean(const double* pos_in, const double* mom_in
   return leapfrog_euclidean_impl(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
                                  n_steps, s, metric_kind, metric_inv, model, h_out, status, n_done,
                                  (cudaStream_t)stream, false);
+}
+
+int mb200_user_target_load(const void* image, int64_t image_bytes, const char* const* names,
+                           int32_t n_names, void** handle) {
+  if (!image || image_bytes <= 0 || !names || !handle)
+    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_names != 2 * N_GENERIC_LAYOUTS)
+    return fail(MB200_ERR_INVALID_ARG, "expected %d kernel names, got %d", 2 * N_GENERIC_LAYOUTS,
+                n_names);
+  UserKernels* u = new UserKernels();
+  cudaError_t e = cudaLibraryLoadData(&u->lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0);
+  if (e != cudaSuccess) {
+    delete u;
+    return fail(MB200_ERR_CUDA, "cudaLibraryLoadData: %s", cudaGetErrorString(e));
+  }
+  for (int i = 0; i < n_names; ++i) {
+    cudaKernel_t k;
+    e = cudaLibraryGetKernel(&k, u->lib, names[i]);
+    if (e != cudaSuccess) {
+      cudaLibraryUnload(u->lib);
+      delete u;
+      return fail(MB200_ERR_CUDA, "cudaLibraryGetKernel(%s): %s", names[i], cudaGetErrorString(e));
+    }
+    (i < N_GENERIC_LAYOUTS ? u->leapfrog[i] : u->eval[i - N_GENERIC_LAYOUTS]) = (const void*)k;
+  }
+  *handle = u;
+  return 0;
+}
+
+int mb200_user_target_unload(void* handle) {
+  if (!handle) return fail(MB200_ERR_INVALID_ARG, "null handle");
+  UserKernels* u = static_cast<UserKernels*>(handle);
+  const cudaError_t e = cudaLibraryUnload(u->lib);
+  delete u;
+  if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "cudaLibraryUnload: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+int mb200_leapfrog_euclidean_user(const double* pos_in, const double* mom_in, double* pos_out,
+                                  double* mom_out, const int32_t* dir, int64_t n_chains,
+                                  int32_t dim, double step_size, const double* step_sizes,
+                                  int32_t n_steps, const int32_t* n_steps_per_chain,
+                                  int32_t n_flows, const double* coefficients,
+                                  int32_t initial_h1_flow_step, int32_t metric_kind,
+                                  const double* metric_inv, const mb200_model* model,
+                                  double* h_out, int32_t* status, int32_t* n_done, void* stream,
+                                  const void* user_target) {
+  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  return leapfrog_euclidean_entry(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
+                                  step_sizes, n_steps, n_steps_per_chain, n_flows, coefficients,
+                                  initial_h1_flow_step, metric_kind, metric_inv, model, h_out,
+                                  status, n_done, (cudaStream_t)stream, false,
+                                  static_cast<const UserKernels*>(user_target));
+}
+
+int mb200_hamiltonian_euclidean_user(const double* pos, const double* mom, int64_t n_chains,
+                                     int32_t dim, int32_t metric_kind, const double* metric_inv,
+                                     const mb200_model* model, double* h_out, void* stream,
+                                     const void* user_target) {
+  if (n_chains == 0 && dim >= 1) return 0;
+  if (!h_out) return fail(MB200_ERR_INVALID_ARG, "h_out is NULL");
+  // zero leapfrog steps, as mb200_hamiltonian_euclidean
+  return mb200_leapfrog_euclidean_user(pos, mom, const_cast<double*>(pos),
+                                       const_cast<double*>(mom), nullptr, n_chains, dim, 0.0,
+                                       nullptr, 0, nullptr, 0, nullptr, 0, metric_kind,
+                                       metric_inv, model, h_out, nullptr, nullptr, stream,
+                                       user_target);
+}
+
+int mb200_euclidean_eval_user(const double* pos, const double* mom, int64_t n_chains, int32_t dim,
+                              int32_t metric_kind, const double* metric_inv,
+                              const mb200_model* model, double* nld_out, double* grad_out,
+                              double* vel_out, double* kin_out, void* stream,
+                              const void* user_target) {
+  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  return euclidean_eval_impl(pos, mom, n_chains, dim, metric_kind, metric_inv, model, nld_out,
+                             grad_out, vel_out, kin_out, (cudaStream_t)stream,
+                             static_cast<const UserKernels*>(user_target));
 }
 
 int64_t mb200_host_scratch_bytes(int64_t n_chains, int32_t dim) {

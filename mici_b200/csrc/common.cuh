@@ -1,7 +1,11 @@
-// Shared device helpers for libmici_b200 (sm_90a).
+// Shared device helpers for libmici_b200 (sm_90a).  Also compiled by NVRTC for user-written
+// targets (csrc/user_target.cuh): NVRTC has no system headers, but declares the vector types
+// and device math functions itself.
 #pragma once
+#ifndef __CUDACC_RTC__
 #include <cuda_runtime.h>
 #include <stdint.h>
+#endif
 
 #include "../../include/mici_b200.h"
 

@@ -19,13 +19,93 @@
 
 namespace mb200 {
 
+// Whole-vector targets (user-written models, user_target.cuh) set `WHOLE_VECTOR = true`: they see
+// a chain's whole position vector in shared memory instead of the pair interface of targets.cuh.
+template <class T, class = void>
+struct IsWholeVector {
+  static constexpr bool value = false;
+};
+template <class T>
+struct IsWholeVector<T, decltype(void(T::WHOLE_VECTOR))> {
+  static constexpr bool value = T::WHOLE_VECTOR;
+};
+
 template <class Target, int KP, int CPW>
 struct LeapfrogGeneric {
   static constexpr int NV = 2 * KP;  // coordinates per lane per chain
+  static constexpr bool WHOLE = IsWholeVector<Target>::value;
+
+  // Staging area of a whole-vector target: q then g, 64 KP doubles each, per warp, after the
+  // CPW * 64 KP doubles per warp of inv_metric_apply (launch_generic / launch_eval size both).
+  // The warp's chains call the target one after the other, so one area per warp suffices.
+  static __device__ __forceinline__ double* whole_stage() {
+    extern __shared__ double smem[];
+    return smem + (size_t)(blockDim.x >> 5) * CPW * 64 * KP + (size_t)(threadIdx.x >> 5) * 128 * KP;
+  }
+  static __device__ __forceinline__ void whole_put_q(int lane, const double (&q)[NV], double* qs) {
+    __syncwarp();
+#pragma unroll
+    for (int k = 0; k < KP; ++k) {
+      const int i = 2 * lane + 64 * k;
+      qs[i] = q[2 * k];
+      qs[i + 1] = q[2 * k + 1];
+    }
+    __syncwarp();
+  }
+  static __device__ __forceinline__ void whole_grad(const Target& t, int dim, int lane,
+                                                    const double (&q)[NV], double (&g)[NV]) {
+    double* qs = whole_stage();
+    double* gs = qs + 64 * KP;
+    whole_put_q(lane, q, qs);
+    t.grad(qs, dim, lane, gs);
+    __syncwarp();
+#pragma unroll
+    for (int k = 0; k < KP; ++k) {
+      const int i = 2 * lane + 64 * k;
+      g[2 * k] = (i < dim) ? gs[i] : 0.0;
+      g[2 * k + 1] = (i + 1 < dim) ? gs[i + 1] : 0.0;
+    }
+  }
+  static __device__ __forceinline__ double whole_nld(const Target& t, int dim, int lane,
+                                                     const double (&q)[NV]) {
+    double* qs = whole_stage();
+    whole_put_q(lane, q, qs);
+    const double l = t.nld(qs, dim, lane);
+    __syncwarp();
+    return l;
+  }
 
   // gradient of l at q (pair layout); all lanes of the warp participate
   static __device__ __forceinline__ void grad(const Target& t, int dim, int lane,
                                               const double (&q)[NV], double (&g)[NV]) {
+    if constexpr (WHOLE) whole_grad(t, dim, lane, q, g);
+    else pair_grad(t, dim, lane, q, g);
+  }
+  // the same gradient, also handing out the target's reduced sums at q (red[NRED + 1]) so that a
+  // caller which needs l(q) at the same position next (a NUTS leaf) does not reduce them again;
+  // a whole-vector target has none
+  static __device__ __forceinline__ void grad_keep(const Target& t, int dim, int lane,
+                                                   const double (&q)[NV], double (&g)[NV],
+                                                   double (&red)[Target::NRED + 1]) {
+    if constexpr (WHOLE) whole_grad(t, dim, lane, q, g);
+    else pair_grad_keep(t, dim, lane, q, g, red);
+  }
+  // l(q) from sums already reduced at this q (grad_keep)
+  static __device__ __forceinline__ double neg_log_dens_with(const Target& t, int dim, int lane,
+                                                             const double (&q)[NV],
+                                                             const double (&red)[Target::NRED + 1]) {
+    if constexpr (WHOLE) return whole_nld(t, dim, lane, q);
+    else return pair_neg_log_dens_with(t, dim, lane, q, red);
+  }
+  static __device__ __forceinline__ double neg_log_dens(const Target& t, int dim, int lane,
+                                                        const double (&q)[NV]) {
+    if constexpr (WHOLE) return whole_nld(t, dim, lane, q);
+    else return pair_neg_log_dens(t, dim, lane, q);
+  }
+
+  // ---- pair interface (targets.cuh)
+  static __device__ __forceinline__ void pair_grad(const Target& t, int dim, int lane,
+                                                   const double (&q)[NV], double (&g)[NV]) {
     double red[Target::NRED + 1];
 #pragma unroll
     for (int r = 0; r < Target::NRED; ++r) red[r] = 0.0;
@@ -47,11 +127,9 @@ struct LeapfrogGeneric {
     }
   }
 
-  // the same gradient, also handing out the target's reduced sums at q (red[NRED + 1]) so that a
-  // caller which needs l(q) at the same position next (a NUTS leaf) does not reduce them again
-  static __device__ __forceinline__ void grad_keep(const Target& t, int dim, int lane,
-                                                   const double (&q)[NV], double (&g)[NV],
-                                                   double (&red)[Target::NRED + 1]) {
+  static __device__ __forceinline__ void pair_grad_keep(const Target& t, int dim, int lane,
+                                                        const double (&q)[NV], double (&g)[NV],
+                                                        double (&red)[Target::NRED + 1]) {
 #pragma unroll
     for (int r = 0; r < Target::NRED + 1; ++r) red[r] = 0.0;
     if (Target::NRED > 0) {
@@ -71,10 +149,9 @@ struct LeapfrogGeneric {
       if (i + 1 >= dim) g[2 * k + 1] = 0.0;
     }
   }
-  // l(q) from sums already reduced at this q (grad_keep)
-  static __device__ __forceinline__ double neg_log_dens_with(const Target& t, int dim, int lane,
-                                                             const double (&q)[NV],
-                                                             const double (&red)[Target::NRED + 1]) {
+  static __device__ __forceinline__ double pair_neg_log_dens_with(
+      const Target& t, int dim, int lane, const double (&q)[NV],
+      const double (&red)[Target::NRED + 1]) {
     double l = 0.0;
 #pragma unroll
     for (int k = 0; k < KP; ++k) {
@@ -84,8 +161,8 @@ struct LeapfrogGeneric {
     return warp_sum(l);
   }
 
-  static __device__ __forceinline__ double neg_log_dens(const Target& t, int dim, int lane,
-                                                        const double (&q)[NV]) {
+  static __device__ __forceinline__ double pair_neg_log_dens(const Target& t, int dim, int lane,
+                                                             const double (&q)[NV]) {
     double red[Target::NRED + 1];
 #pragma unroll
     for (int r = 0; r < Target::NRED; ++r) red[r] = 0.0;

@@ -47,6 +47,15 @@ class ExtensionNotBuiltError(Error):
     """libmici_b200.so is missing or cannot be loaded: there is no CPU fallback."""
 
 
+class TargetCompileError(Error):
+    """A user-written target (``mici_b200.targets.CudaTarget``) does not compile; ``log`` holds
+    the NVRTC log, whose line numbers are the user source's."""
+
+    def __init__(self, msg, log=""):
+        super().__init__(msg)
+        self.log = log
+
+
 # per-chain status codes written by the kernels (include/mici_b200.h)
 STATUS_OK = 0
 STATUS_CONVERGENCE = 1

@@ -42,6 +42,7 @@ _FUSED_PROJECTION_SOLVERS = (
     solve_projection_onto_manifold_newton_with_line_search,
 )
 from .states import ChainState
+from .targets import CudaTarget, user_handle
 from .systems import (
     ConstrainedEuclideanMetricSystem,
     EuclideanMetricSystem,
@@ -256,14 +257,19 @@ class TractableFlowIntegrator(Integrator):
         eps, eps_t, ns, max_n = _step_args(self.step_size, n_steps, n, dev)
         coefs, n_flows = _coefficients_arg(self.coefficients)
         model = sysm._model(dev)
-        rc = _lib.load().mb200_leapfrog_euclidean(
+        args = (
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
             n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), n_flows, coefs,
             1 if self.initial_h1_flow_step else 0, sysm.metric.kind,
             _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model), _lib.ptr(h),
             _lib.ptr(status), _lib.ptr(n_done), _lib.current_stream_ptr(dev),
         )
-        _lib.check(rc, "mb200_leapfrog_euclidean")
+        user = user_handle(sysm.target)
+        if user is None:
+            _lib.check(_lib.load().mb200_leapfrog_euclidean(*args), "mb200_leapfrog_euclidean")
+        else:  # user-written target: general-dimension kernel of its run-time compiled image
+            _lib.check(_lib.load().mb200_leapfrog_euclidean_user(*args, user),
+                       "mb200_leapfrog_euclidean_user")
 
 
 def _step_args(step_size, n_steps, n, dev):
@@ -364,6 +370,7 @@ class LeapfrogIntegrator(TractableFlowIntegrator):
                         n_chunks):
         tensors = (pos, mom, out_pos, out_mom)
         if (isinstance(self.system, GaussianEuclideanMetricSystem)
+                or isinstance(self.system.target, CudaTarget)
                 or _is_per_chain(self.step_size, n_steps) or self.step_size is None
                 or any(t.device.type != "cpu" or t.dtype != torch.float64 or not t.is_contiguous()
                        for t in tensors)

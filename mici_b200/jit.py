@@ -1,0 +1,234 @@
+"""Run-time compilation of user-written targets with NVRTC (``targets.CudaTarget``).
+
+A user target is two CUDA device functions (contract: ``csrc/user_target.cuh``).  They are
+compiled together with the engine's general-dimension Euclidean kernels
+(``csrc/leapfrog_generic.cuh``) into one sm_90a CUBIN, which ``libmici_b200.so`` loads
+(``mb200_user_target_load``).  NVRTC is driven through ``ctypes``; it needs no GPU, so compiling
+works anywhere.  The library itself never links NVRTC.
+
+Compiled images and loaded handles live in one process-wide cache keyed by a hash of the
+headers, the user source, the options and the NVRTC version (nothing is written to disk), so
+that system and integrator objects hold only the source and survive ``deepcopy`` / pickling.
+"""
+
+from __future__ import annotations
+
+import ctypes
+import glob
+import hashlib
+import os
+import threading
+
+from .errors import Error, TargetCompileError
+
+_PKG = os.path.dirname(os.path.abspath(__file__))
+CSRC = os.path.join(_PKG, "csrc")
+INCLUDE = os.path.join(os.path.dirname(_PKG), "include")
+ARCH = "sm_90a"
+# -fmad=false as the library (csrc/Makefile): products and sums round as in NumPy.
+# -default-device: the C prototypes of include/mici_b200.h become (unused) device declarations.
+OPTIONS = ("-arch=" + ARCH, "-std=c++17", "-fmad=false", "-default-device")
+
+# (KP, CPW) of the general-dimension kernel, in the kernel-table order of mb200_user_target_load
+LAYOUTS = ((1, 4), (2, 4), (4, 2), (8, 1), (16, 1))
+NAME_EXPRESSIONS = tuple(
+    [f"&mb200::leapfrog_generic_kernel<mb200::UserTarget, {kp}, {cpw}, false>" for kp, cpw in LAYOUTS]
+    + [f"&mb200::euclidean_eval_kernel<mb200::UserTarget, {kp}>" for kp, _ in LAYOUTS]
+)
+
+_lock = threading.Lock()
+_nvrtc = None
+_images = {}   # key -> (cubin bytes, lowered names)
+_handles = {}  # key -> loaded library handle (ctypes.c_void_p)
+# (source, name) -> key / handle: a repeat lookup, once per launch of a user target, is one dict
+# access; the headers are hashed and NVRTC's version read once per process (_static_key)
+_keys = {}
+_loaded = {}
+_static = None
+stats = {"compiles": 0, "hits": 0}
+
+
+def _candidates():
+    """``libnvrtc.so.12`` locations in search order: the ``nvidia-cuda-nvrtc`` wheel that torch
+    depends on, the default loader path, ``$CUDA_HOME/lib64``."""
+    out = []
+    try:
+        import nvidia.cuda_nvrtc as pkg  # noqa: PLC0415
+
+        for d in pkg.__path__:
+            out.append(os.path.join(d, "lib", "libnvrtc.so.12"))
+    except ImportError:
+        out.append("<nvidia.cuda_nvrtc package not installed>")
+    out.append("libnvrtc.so.12")
+    cuda_home = os.environ.get("CUDA_HOME", "/usr/local/cuda")
+    out.append(os.path.join(cuda_home, "lib64", "libnvrtc.so.12"))
+    return out
+
+
+def nvrtc():
+    """The loaded NVRTC library (``ctypes.CDLL``); its path is ``nvrtc()._name``."""
+    global _nvrtc  # noqa: PLW0603
+    with _lock:
+        if _nvrtc is None:
+            tried = []
+            for path in _candidates():
+                if path.startswith("<"):
+                    tried.append(path)
+                    continue
+                try:
+                    lib = ctypes.CDLL(path)
+                except OSError as e:
+                    tried.append(f"{path}: {e}")
+                    continue
+                _declare(lib)
+                _nvrtc = lib
+                break
+            else:
+                raise Error("cannot load NVRTC (libnvrtc.so.12); tried:\n  " + "\n  ".join(tried))
+    return _nvrtc
+
+
+def _declare(lib):
+    p, sz = ctypes.c_void_p, ctypes.c_size_t
+    pp = ctypes.POINTER(ctypes.c_void_p)
+    sigs = {
+        "nvrtcVersion": [ctypes.POINTER(ctypes.c_int)] * 2,
+        "nvrtcGetErrorString": [ctypes.c_int],
+        "nvrtcCreateProgram": [pp, ctypes.c_char_p, ctypes.c_char_p, ctypes.c_int, p, p],
+        "nvrtcDestroyProgram": [pp],
+        "nvrtcAddNameExpression": [p, ctypes.c_char_p],
+        "nvrtcCompileProgram": [p, ctypes.c_int, p],
+        "nvrtcGetProgramLogSize": [p, ctypes.POINTER(sz)],
+        "nvrtcGetProgramLog": [p, ctypes.c_char_p],
+        "nvrtcGetCUBINSize": [p, ctypes.POINTER(sz)],
+        "nvrtcGetCUBIN": [p, ctypes.c_char_p],
+        "nvrtcGetLoweredName": [p, ctypes.c_char_p, ctypes.POINTER(ctypes.c_char_p)],
+    }
+    for name, args in sigs.items():
+        fn = getattr(lib, name)
+        fn.argtypes = args
+        fn.restype = ctypes.c_char_p if name == "nvrtcGetErrorString" else ctypes.c_int
+
+
+def version():
+    """``(major, minor)`` of the loaded NVRTC."""
+    lib = nvrtc()
+    major, minor = ctypes.c_int(), ctypes.c_int()
+    _ok(lib.nvrtcVersion(ctypes.byref(major), ctypes.byref(minor)), "nvrtcVersion")
+    return major.value, minor.value
+
+
+def _ok(rc, what):
+    if rc != 0:
+        msg = nvrtc().nvrtcGetErrorString(rc).decode()
+        raise Error(f"{what} failed: {msg}")
+
+
+def _headers_digest():
+    h = hashlib.sha256()
+    for path in sorted(glob.glob(os.path.join(CSRC, "*.cuh"))) + [
+            os.path.join(INCLUDE, "mici_b200.h")]:
+        with open(path, "rb") as f:
+            h.update(os.path.basename(path).encode() + b"\0" + f.read())
+    return h.hexdigest()
+
+
+def translation_unit(source, name="user_target"):
+    """The program NVRTC compiles: the engine header, then the user source with its own line
+    numbers (``#line``), so that compile errors point at the user's lines."""
+    return f'#include "user_target.cuh"\n#line 1 "{name}.cu"\n{source}\n'
+
+
+def _static_key():
+    """The part of every cache key that is fixed for the process: the header contents, the
+    options and the NVRTC version."""
+    global _static  # noqa: PLW0603
+    if _static is None:
+        _static = "\0".join([_headers_digest(), *OPTIONS, "%d.%d" % version()])
+    return _static
+
+
+def cache_key(source, name="user_target"):
+    return hashlib.sha256("\0".join([_static_key(), name, source]).encode()).hexdigest()
+
+
+def compile_target(source, name="user_target"):
+    """Compile a user target; returns ``(key, cubin, lowered kernel names)``, from the process
+    cache when the same source was compiled before.  Raises ``TargetCompileError`` with the
+    NVRTC log on failure."""
+    with _lock:
+        key = _keys.get((source, name))
+        if key is not None:
+            stats["hits"] += 1
+            return key, *_images[key]
+    key = cache_key(source, name)
+    with _lock:
+        if key in _images:  # the same program under another (source, name) spelling
+            stats["hits"] += 1
+            _keys[(source, name)] = key
+            return key, *_images[key]
+    cubin, names = _compile(source, name)
+    with _lock:
+        _images.setdefault(key, (cubin, names))
+        _keys[(source, name)] = key
+        stats["compiles"] += 1
+        return key, *_images[key]
+
+
+def _compile(source, name):
+    lib = nvrtc()
+    prog = ctypes.c_void_p()
+    src = translation_unit(source, name).encode()
+    _ok(lib.nvrtcCreateProgram(ctypes.byref(prog), src, f"{name}_tu.cu".encode(), 0, None, None),
+        "nvrtcCreateProgram")
+    try:
+        for expr in NAME_EXPRESSIONS:
+            _ok(lib.nvrtcAddNameExpression(prog, expr.encode()), "nvrtcAddNameExpression")
+        opts = [o.encode() for o in OPTIONS] + [f"-I{CSRC}".encode(), f"-I{INCLUDE}".encode()]
+        argv = (ctypes.c_char_p * len(opts))(*opts)
+        rc = lib.nvrtcCompileProgram(prog, len(opts), ctypes.cast(argv, ctypes.c_void_p))
+        log_size = ctypes.c_size_t()
+        _ok(lib.nvrtcGetProgramLogSize(prog, ctypes.byref(log_size)), "nvrtcGetProgramLogSize")
+        log = ctypes.create_string_buffer(max(log_size.value, 1))
+        _ok(lib.nvrtcGetProgramLog(prog, log), "nvrtcGetProgramLog")
+        log = log.value.decode("utf-8", "replace")
+        if rc != 0:
+            err = lib.nvrtcGetErrorString(rc).decode()
+            raise TargetCompileError(f"user target {name!r} does not compile ({err}):\n{log}",
+                                     log=log)
+        size = ctypes.c_size_t()
+        _ok(lib.nvrtcGetCUBINSize(prog, ctypes.byref(size)), "nvrtcGetCUBINSize")
+        cubin = ctypes.create_string_buffer(size.value)
+        _ok(lib.nvrtcGetCUBIN(prog, cubin), "nvrtcGetCUBIN")
+        names = []
+        for expr in NAME_EXPRESSIONS:
+            lowered = ctypes.c_char_p()
+            _ok(lib.nvrtcGetLoweredName(prog, expr.encode(), ctypes.byref(lowered)),
+                "nvrtcGetLoweredName")
+            names.append(lowered.value.decode())
+        return cubin.raw, tuple(names)
+    finally:
+        lib.nvrtcDestroyProgram(ctypes.byref(prog))
+
+
+def load_target(source, name="user_target"):
+    """Handle of the loaded image of a user target (``mb200_user_target_load``), compiled and
+    loaded once per process."""
+    from . import _lib  # noqa: PLC0415
+
+    with _lock:
+        handle = _loaded.get((source, name))
+    if handle is not None:
+        return handle
+    key, cubin, names = compile_target(source, name)
+    with _lock:
+        handle = _handles.get(key)
+        if handle is None:
+            lib = _lib.load()
+            arr = (ctypes.c_char_p * len(names))(*[n.encode() for n in names])
+            handle = ctypes.c_void_p()
+            _lib.check(lib.mb200_user_target_load(cubin, len(cubin), arr, len(names),
+                                                  ctypes.byref(handle)), "mb200_user_target_load")
+            _handles[key] = handle
+        _loaded[(source, name)] = handle
+    return handle

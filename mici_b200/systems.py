@@ -29,6 +29,7 @@ from . import _lib
 from .errors import LinAlgError
 from .targets import (
     RMETRIC_SOFTABS,
+    CudaTarget,
     FunnelFisherMetric,
     HadamardMetric,
     NealFunnel,
@@ -37,6 +38,7 @@ from .targets import (
     QuadraticScalarMetric,
     Rank1Metric,
     Target,
+    user_handle,
 )
 
 METRIC_IDENTITY, METRIC_DIAGONAL, METRIC_DENSE = 0, 1, 2
@@ -164,13 +166,20 @@ def _dir_tensor(d, n, device):
 class System:
     """Base class (systems.py:39-229): holds the target model and builds ``mb200_model``."""
 
+    # whether a user-written `CudaTarget` may drive the system (its kernels need only l and grad l)
+    _user_targets = False
+
     def __init__(self, neg_log_dens, *, grad_neg_log_dens=None, backend=None):
         if not isinstance(neg_log_dens, Target):
             msg = (
                 "mici_b200 systems take a `mici_b200.targets.Target` instance as `neg_log_dens` "
-                "(models are compiled into the CUDA library); Python callables are not supported."
+                "(a registry model, or a `CudaTarget` written in CUDA C++); Python callables are "
+                "not supported."
             )
             raise TypeError(msg)
+        if isinstance(neg_log_dens, CudaTarget) and not type(self)._user_targets:
+            raise TypeError(f"{type(self).__name__} does not take a CudaTarget: user targets run "
+                            "on EuclideanMetricSystem.")
         if grad_neg_log_dens is not None or backend is not None:
             raise ValueError("Derivatives are fused into the kernels; pass neither "
                              "`grad_neg_log_dens` nor `backend`.")
@@ -228,6 +237,8 @@ class EuclideanMetricSystem(TractableFlowSystem):
     in systems.py:332-346.  Assignable (adapters set it: adapters.py:513, 642).
     """
 
+    _user_targets = True
+
     def __init__(self, neg_log_dens, *, metric=None, grad_neg_log_dens=None, backend=None):
         super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
         self.metric = metric
@@ -256,18 +267,23 @@ class EuclideanMetricSystem(TractableFlowSystem):
             out["vel"] = torch.empty_like(pos)
         if kin:
             out["kin"] = torch.empty(n, dtype=torch.float64, device=dev)
+        user = None
         if nld or grad:
             model = self._model(dev)
+            user = user_handle(self.target)
         else:  # M^-1 p and p.M^-1 p do not involve the target (constrained targets have no
             model = _lib.Model()  # Euclidean-eval functor): neutral model
             model.target_id = 0
-        rc = lib.mb200_euclidean_eval(
+        args = (
             _lib.ptr(pos), _lib.ptr(mom), n, dim, self._metric.kind,
             _lib.ptr(self._metric.inv_device(dev)), ctypes.byref(model),
             _lib.ptr(out.get("nld")), _lib.ptr(out.get("grad")), _lib.ptr(out.get("vel")),
             _lib.ptr(out.get("kin")), _lib.current_stream_ptr(dev),
         )
-        _lib.check(rc, "mb200_euclidean_eval")
+        if user is None:
+            _lib.check(lib.mb200_euclidean_eval(*args), "mb200_euclidean_eval")
+        else:
+            _lib.check(lib.mb200_euclidean_eval_user(*args, user), "mb200_euclidean_eval_user")
         if single:
             out = {k: v[0] for k, v in out.items()}
         return {k: _like_input(state.pos, v) for k, v in out.items()}  # NumPy in -> NumPy out
@@ -305,12 +321,17 @@ class EuclideanMetricSystem(TractableFlowSystem):
         dev = pos.device
         h = torch.empty(n, dtype=torch.float64, device=dev)
         model = self._model(dev)
-        rc = _lib.load().mb200_hamiltonian_euclidean(
+        args = (
             _lib.ptr(pos.contiguous()), _lib.ptr(mom.contiguous()), n, dim, self._metric.kind,
             _lib.ptr(self._metric.inv_device(dev)), ctypes.byref(model), _lib.ptr(h),
             _lib.current_stream_ptr(dev),
         )
-        _lib.check(rc, "mb200_hamiltonian_euclidean")
+        user = user_handle(self.target)
+        if user is None:
+            _lib.check(_lib.load().mb200_hamiltonian_euclidean(*args), "mb200_hamiltonian_euclidean")
+        else:
+            _lib.check(_lib.load().mb200_hamiltonian_euclidean_user(*args, user),
+                       "mb200_hamiltonian_euclidean_user")
         return _like_input(state.pos, h[0] if single else h)
 
     def h1_flow(self, state, dt):
@@ -359,6 +380,8 @@ class GaussianEuclideanMetricSystem(EuclideanMetricSystem):
     ``h2_flow`` is the exact rotation of ``(q, p)`` in the eigenbasis of ``M``.  The tractable-
     flow integrators (leapfrog, symmetric compositions) drive it through
     ``mb200_leapfrog_gaussian_euclidean``."""
+
+    _user_targets = False
 
     def h2(self, state):
         """``q.q/2 + p.M^-1 p/2`` (systems.py:450-453)."""
@@ -439,6 +462,8 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
     its gradient through the constraint's matrix-Hessian product (systems.py:853-861, 1024-1031),
     fused into the kernels.
     """
+
+    _user_targets = False
 
     def __init__(self, neg_log_dens, constr=None, *, metric=None, dens_wrt_hausdorff=True,
                  grad_neg_log_dens=None, jacob_constr=None, backend=None):

@@ -4,7 +4,8 @@ The reference accepts arbitrary Python callables for ``neg_log_dens`` and its de
 (``src/mici/systems.py:88-95``).  A fused GPU gradient cannot, so the engine ships a closed
 registry of models compiled into ``libmici_b200.so`` (``mici_b200/csrc/targets.cuh``); an
 instance of one of these classes is what is passed as ``neg_log_dens=`` to the systems in
-``mici_b200.systems``.  Instances only carry ids and parameters -- no host arithmetic.
+``mici_b200.systems``.  Instances only carry ids and parameters -- no host arithmetic.  Other
+models are written by the user in CUDA C++ and compiled at run time (``CudaTarget``).
 """
 
 from __future__ import annotations
@@ -19,6 +20,7 @@ TARGET_TORUS = 4
 TARGET_SPHERE = 5
 TARGET_MULTI_SPHERE = 6
 TARGET_QUARTIC = 7
+TARGET_USER = 64  # MB200_TARGET_USER: CudaTarget, compiled at run time
 
 RMETRIC_SOFTABS = 0
 RMETRIC_RANK1 = 1
@@ -137,6 +139,70 @@ class Sphere(Target):
 
     def __init__(self, dim):
         super().__init__(dim)
+
+
+class CudaTarget(Target):
+    """A user-written model: CUDA C++ source defining
+
+        __device__ double neg_log_dens(const mb200::Chain& c);
+        __device__ void grad_neg_log_dens(const mb200::Chain& c, double* g);
+
+    (contract and rules: ``mici_b200/csrc/user_target.cuh``), compiled at run time with NVRTC
+    together with the engine's general-dimension Euclidean kernels (``mici_b200.jit``).  ``params``
+    (at most 8 scalars) reach the functions as ``c.params``, ``aux`` (any array convertible to
+    fp64, e.g. a data matrix) as the device array ``c.aux``.  Runs on ``EuclideanMetricSystem``
+    with any fixed metric, ``dim <= 1024``.
+
+    The source compiles on first use (``compile()`` compiles now).  The instance holds only
+    source, params and aux; the compiled image lives in a process-wide cache, so systems and
+    integrators holding a ``CudaTarget`` survive ``deepcopy`` and pickling."""
+
+    target_id = TARGET_USER
+
+    def __init__(self, dim, source, params=(), aux=None, name=None):
+        if not isinstance(source, str):
+            raise ValueError("`source` must be a string of CUDA C++.")
+        dim = int(dim)
+        if not 1 <= dim <= 1024:
+            raise ValueError(f"CudaTarget dimension must be in [1, 1024], got {dim}.")
+        try:
+            params = tuple(float(x) for x in params)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"`params` must be an iterable of scalars: {e}") from e
+        if len(params) > 8:
+            raise ValueError(f"CudaTarget takes at most 8 params, got {len(params)}.")
+        if aux is not None:
+            try:
+                aux = np.ascontiguousarray(aux, dtype=np.float64)
+            except (TypeError, ValueError) as e:
+                raise ValueError(f"`aux` cannot be converted to a float64 array: {e}") from e
+        super().__init__(dim, params, aux)
+        self.source = source
+        self.name = "user_target" if name is None else str(name)
+        if not self.name.isidentifier():
+            raise ValueError("`name` must be a valid identifier.")
+
+    def compile(self):
+        """Compile now (raises ``mici_b200.errors.TargetCompileError``); returns ``self``."""
+        from . import jit  # noqa: PLC0415
+
+        jit.compile_target(self.source, self.name)
+        return self
+
+    def handle(self):
+        """The loaded device image (``mb200_user_target_load``) of this source, from the process
+        cache."""
+        from . import jit  # noqa: PLC0415
+
+        return jit.load_target(self.source, self.name)
+
+    def __repr__(self):
+        return f"CudaTarget(dim={self.dim}, name={self.name!r}, params={self.params})"
+
+
+def user_handle(target):
+    """The loaded image of a ``CudaTarget``, or ``None`` for a registry target."""
+    return target.handle() if isinstance(target, CudaTarget) else None
 
 
 class Rank1Metric:

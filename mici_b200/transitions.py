@@ -231,6 +231,7 @@ class DynamicIntegrationTransition:
                  termination_criterion=riemannian_no_u_turn_criterion,
                  do_extra_subtree_checks=True):
         from .integrators import LeapfrogIntegrator  # noqa: PLC0415
+        from .targets import CudaTarget  # noqa: PLC0415
         from .systems import (  # noqa: PLC0415
             ConstrainedEuclideanMetricSystem,
             EuclideanMetricSystem,
@@ -247,11 +248,12 @@ class DynamicIntegrationTransition:
             raise ValueError("Only the two no-U-turn criteria of this module are fused.")
         # LeapfrogIntegrator on a plain EuclideanMetricSystem: whole transitions in ONE launch
         # (mb200_nuts_euclidean).  Every other pair (constrained, implicit, compositions,
-        # Gaussian splitting): lock-step leaves through the integrator's own kernels with the
-        # tree bookkeeping in the mb200_nuts_generic_* kernels.
+        # Gaussian splitting, user-written targets): lock-step leaves through the integrator's own
+        # kernels with the tree bookkeeping in the mb200_nuts_generic_* kernels.
         self._fused = type(integrator) is LeapfrogIntegrator and isinstance(
             system, EuclideanMetricSystem) and not isinstance(
-            system, (ConstrainedEuclideanMetricSystem, GaussianEuclideanMetricSystem))
+            system, (ConstrainedEuclideanMetricSystem, GaussianEuclideanMetricSystem)) \
+            and not isinstance(system.target, CudaTarget)
         self.system = system
         self.integrator = integrator
         self.max_tree_depth = int(max_tree_depth)
