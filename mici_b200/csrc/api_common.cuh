@@ -5,8 +5,10 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <type_traits>
 
 #include "common.cuh"
+#include "targets.cuh"
 
 namespace mb200 {
 
@@ -19,6 +21,12 @@ inline int fail(int code, const char* fmt, ...) {
   va_end(ap);
   return code;
 }
+
+// a type as a value (also keeps a parameter out of template argument deduction)
+template <class T>
+struct TypeTag {
+  using type = T;
+};
 
 inline int check_launch(const char* what) {
   cudaError_t e = cudaGetLastError();
@@ -100,11 +108,137 @@ struct DgScratch {
   }
 };
 
-// implemented in api_dmma.cu (tensor-core leapfrog); MB200_ERR_UNSUPPORTED = outside its domain
-int leapfrog_dmma_dispatch(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                           const int32_t* dir, const double* step_sizes, int64_t n, int dim,
-                           double eps, int n_steps, const double* minv, const ModelArgs& m,
-                           double* h_out, int32_t* status, int32_t* n_done, cudaStream_t st);
+// ---- Euclidean family: which kernel serves a model (api_euclid.cu, api_nuts.cu, api_dmma.cu) ----
+
+// Arguments of one Euclidean leapfrog launch (zero steps evaluate the Hamiltonian only).
+// allow_k1: the caller lets the tensor-core kernel K1 serve the call (mb200_leapfrog_euclidean
+// with the default leapfrog schedule); k1_serves() decides whether it does.
+struct EuclidArgs {
+  const double *q_in, *p_in;
+  double *q_out, *p_out;
+  const int32_t* dir;
+  int64_t n;
+  int dim;
+  double eps;
+  int n_steps;
+  FlowSchedule sched;
+  int metric_kind;
+  const double* minv;
+  ModelArgs m;
+  double* h_out;
+  int32_t *status, *n_done;
+  cudaStream_t st;
+  bool allow_k1;
+};
+
+// K1's domain: one trajectory length for every chain, n_steps > 0, a dense metric,
+// 8 <= dim <= 128, a registry target, and per-chain step sizes or a finite non-zero eps (K1 stages
+// eps * M^-1 in shared memory)
+inline bool k1_serves(int metric_kind, int dim, double eps, const double* step_sizes, int n_steps,
+                      const int32_t* n_steps_pc, int target_id) {
+  return n_steps_pc == nullptr && n_steps > 0 && metric_kind == MB200_METRIC_DENSE && dim >= 8 &&
+         dim <= 128 && (step_sizes != nullptr || (eps != 0.0 && isfinite(eps))) &&
+         (target_id == MB200_TARGET_STD_GAUSSIAN || target_id == MB200_TARGET_NEAL_FUNNEL ||
+          target_id == MB200_TARGET_BANANA);
+}
+
+// K1 for one registry target (api_dmma.cu)
+template <class Target>
+int k1_launch(const EuclidArgs& a);
+
+// (KP, CPW) of the warp-per-chain Euclidean kernels -- K1g, evaluation, fused NUTS and the generic
+// NUTS steps -- by dimension: layout l serves dim <= max_dim.  A user target's kernel table
+// (mb200_user_target_load) is in this order, and mici_b200/jit.py LAYOUTS lists it: keep the two
+// in step.
+struct EuLayout {
+  int max_dim, kp, cpw;
+};
+constexpr EuLayout EU_LAYOUTS[] = {{64, 1, 4}, {128, 2, 4}, {256, 4, 2}, {512, 8, 1}, {1024, 16, 1}};
+constexpr int N_EU_LAYOUTS = sizeof(EU_LAYOUTS) / sizeof(EU_LAYOUTS[0]);
+
+// f(std::integral_constant<int, l>()) for the layout l of `dim`
+template <int L = 0, class F>
+int with_layout(int dim, const F& f) {
+  if constexpr (L == N_EU_LAYOUTS)
+    return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported", dim);
+  else
+    return dim <= EU_LAYOUTS[L].max_dim ? f(std::integral_constant<int, L>())
+                                        : with_layout<L + 1>(dim, f);
+}
+
+// Starts `kern` on min(blocks, cap) CTAs of `threads` threads with `smem` bytes of dynamic shared
+// memory (opted in above the default 48 KB); cap is `per_sm` CTAs per SM, or as many as fit when
+// per_sm == 0.  A failure reads "<name>: <CUDA error>".
+template <class... P>
+int eu_launch(void (*kern)(P...), const char* name, int64_t blocks, int per_sm, int threads,
+              size_t smem, cudaStream_t st, typename TypeTag<P>::type... args) {
+  const void* k = (const void*)kern;
+  cudaError_t e = cudaSuccess;
+  if (smem > 48 * 1024)
+    e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e == cudaSuccess && per_sm == 0) {
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, threads, smem);
+    if (per_sm < 1) per_sm = 1;
+  }
+  if (e == cudaSuccess) {
+    const int64_t cap = (int64_t)num_sms() * per_sm;
+    void* argv[] = {&args...};
+    e = cudaLaunchKernel(k, dim3((unsigned)(blocks < cap ? blocks : cap)), dim3(threads), argv,
+                         smem, st);
+  }
+  if (e != cudaSuccess) {
+    cudaGetLastError();  // reported here: clear it from the runtime's error state
+    return fail(MB200_ERR_CUDA, "%s: %s", name, cudaGetErrorString(e));
+  }
+  return check_launch(name);
+}
+
+// the metric arguments every Euclidean entry point takes
+inline int eu_check_metric(int metric_kind, const double* minv) {
+  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
+  if (metric_kind != MB200_METRIC_IDENTITY && !minv)
+    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
+  return 0;
+}
+
+enum class EuOp { Leapfrog, Eval, Nuts };
+
+// Which kernel serves a Euclidean model, for every operation L::op.  Checks the model the same way
+// whatever the operation, picks the route, and hands the target type and the layout to `l`:
+//   l.k1<Target>()        K1, the tensor-core leapfrog (l.k1_ok: k1_serves)
+//   l.dmma<Target, L>()   fused NUTS in lock-step on the tensor pipe (dense metric, 8 <= dim <= 128)
+//   l.warp<Target, L>()   the library's warp-per-chain kernel of the operation
+//   l.image(L)            the same kernel from the loaded user-target image l.user
+template <class L>
+int eu_dispatch(const ModelArgs& m, int dim, int metric_kind, const L& l) {
+  if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
+    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
+  if constexpr (L::op != EuOp::Nuts) {
+    if (l.user != nullptr) {
+      if (m.target_id != MB200_TARGET_USER)
+        return fail(MB200_ERR_INVALID_ARG,
+                    "user-target entry point needs target_id MB200_TARGET_USER");
+      return with_layout(dim, [&](auto lay) { return l.image(lay.value); });
+    }
+  }
+  auto route = [&](auto target) {
+    using Target = typename decltype(target)::type;
+    if constexpr (L::op == EuOp::Leapfrog)
+      if (l.k1_ok()) return l.template k1<Target>();
+    return with_layout(dim, [&](auto lay) {
+      constexpr int LAY = decltype(lay)::value;
+      if constexpr (L::op == EuOp::Nuts && EU_LAYOUTS[LAY].kp <= 2)
+        if (metric_kind == MB200_METRIC_DENSE && dim >= 8) return l.template dmma<Target, LAY>();
+      return l.template warp<Target, LAY>();
+    });
+  };
+  switch (m.target_id) {
+    case MB200_TARGET_STD_GAUSSIAN: return route(TypeTag<StdGaussianTarget>());
+    case MB200_TARGET_NEAL_FUNNEL: return route(TypeTag<NealFunnelTarget>());
+    case MB200_TARGET_BANANA: return route(TypeTag<BananaTarget>());
+  }
+  return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Euclidean systems", m.target_id);
+}
 
 // Arguments of one implicit-integrator launch on a Riemannian system (leapfrog or midpoint steps;
 // zero steps evaluate the Hamiltonian only).  ws / ws_bytes: the caller's workspace, or NULL.

@@ -101,86 +101,17 @@ static bool is_pageable(const void* ptr) {
   return a.type == cudaMemoryTypeUnregistered;
 }
 
-// One launch of the general-dimension kernel `kern` (a leapfrog_generic_kernel<Target, KP, CPW,
-// GAUSS> of the library or of a user-target image).  whole_vector: the target stages each chain's
-// position and gradient in shared memory (user_target.cuh), 2 * 64 KP doubles per warp more.
-static int launch_generic(const void* kern, int kp, int cpw, bool whole_vector,
-                          const double* q_in, const double* p_in, double* q_out, double* p_out,
-                          const int32_t* dir, int64_t n, int dim, double eps, int n_steps,
-                          const FlowSchedule& sched, int metric_kind, const double* minv, const ModelArgs& m, double* h_out,
-                          int32_t* status, int32_t* n_done, cudaStream_t st) {
-  constexpr int WARPS = 4;
-  const size_t smem = (size_t)WARPS * (cpw + (whole_vector ? 2 : 0)) * 64 * kp * sizeof(double);
-  if (smem > 48 * 1024) {
-    cudaError_t e =
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  }
-  const int64_t groups = (n + cpw - 1) / cpw;
-  int64_t blocks = (groups + WARPS - 1) / WARPS;
-  const int64_t cap = (int64_t)num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  if (blocks < 1) blocks = 1;
-  FlowSchedule sc = sched;
-  ModelArgs ma = m;
-  void* args[] = {&q_in, &p_in, &q_out, &p_out, &dir, &n, &dim, &eps, &n_steps, &sc,
-                  &metric_kind, &minv, &ma, &h_out, &status, &n_done};
-  const cudaError_t e =
-      cudaLaunchKernel(kern, dim3((unsigned)blocks), dim3(WARPS * 32), args, smem, st);
-  if (e != cudaSuccess) {
-    cudaGetLastError();  // reported here: clear it from the runtime's error state
-    return fail(MB200_ERR_CUDA, "leapfrog_generic_kernel: %s", cudaGetErrorString(e));
-  }
-  return check_launch("leapfrog_generic_kernel");
-}
-
-// (KP, CPW) of the general-dimension kernel by dimension, in the order of a user target's kernel
-// table (mb200_user_target_load)
-constexpr int N_GENERIC_LAYOUTS = 5;
-constexpr int GENERIC_KP[N_GENERIC_LAYOUTS] = {1, 2, 4, 8, 16};
-constexpr int GENERIC_CPW[N_GENERIC_LAYOUTS] = {4, 4, 2, 1, 1};
-static int generic_layout(int dim) {
-  if (dim <= 64) return 0;
-  if (dim <= 128) return 1;
-  if (dim <= 256) return 2;
-  if (dim <= 512) return 3;
-  if (dim <= 1024) return 4;
-  return -1;
-}
-
 // A loaded user-target image (mb200_user_target_load): its general-dimension leapfrog kernels
 // leapfrog_generic_kernel<UserTarget, KP, CPW, false> and evaluation kernels
-// euclidean_eval_kernel<UserTarget, KP>, one per layout of generic_layout().
+// euclidean_eval_kernel<UserTarget, KP>, one per layout of EU_LAYOUTS.  Their parameters are those
+// of the library's own instantiations.
+using LeapfrogKernel = decltype(&leapfrog_generic_kernel<StdGaussianTarget, 1, 4, false>);
+using EvalKernel = decltype(&euclidean_eval_kernel<StdGaussianTarget, 1>);
 struct UserKernels {
   cudaLibrary_t lib;
-  const void* leapfrog[N_GENERIC_LAYOUTS];
-  const void* eval[N_GENERIC_LAYOUTS];
+  LeapfrogKernel leapfrog[N_EU_LAYOUTS];
+  EvalKernel eval[N_EU_LAYOUTS];
 };
-
-template <class Target>
-static int dispatch_generic_dim(const double* q_in, const double* p_in, double* q_out,
-                                double* p_out, const int32_t* dir, int64_t n, int dim, double eps,
-                                int n_steps, const FlowSchedule& sched, int metric_kind, const double* minv,
-                                const ModelArgs& m, double* h_out, int32_t* status,
-                                int32_t* n_done, cudaStream_t st) {
-#define MB200_GEN(L)                                                                          \
-  {                                                                                           \
-    constexpr int KP = GENERIC_KP[L], CPW = GENERIC_CPW[L];                                   \
-    const void* kern = sched.gaussian ? (const void*)leapfrog_generic_kernel<Target, KP, CPW, true> \
-                                      : (const void*)leapfrog_generic_kernel<Target, KP, CPW, false>; \
-    return launch_generic(kern, KP, CPW, false, q_in, p_in, q_out, p_out, dir, n, dim, eps,   \
-                          n_steps, sched, metric_kind, minv, m, h_out, status, n_done, st);   \
-  }
-  switch (generic_layout(dim)) {
-    case 0: MB200_GEN(0);
-    case 1: MB200_GEN(1);
-    case 2: MB200_GEN(2);
-    case 3: MB200_GEN(3);
-    case 4: MB200_GEN(4);
-  }
-#undef MB200_GEN
-  return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported by the Euclidean leapfrog", dim);
-}
 
 // Splitting schedule of the C-ABI arguments: n_flows (odd) coefficients alternating a, b, ..., a
 // with a = h1_flow (kick) if initial_h1_flow_step else h2_flow (drift) (integrators.py:268-281);
@@ -205,56 +136,78 @@ static int make_schedule(FlowSchedule& s, int n_flows, const double* coefficient
   return 0;
 }
 
-static int leapfrog_euclidean_impl(const double* q_in, const double* p_in, double* q_out,
-                                   double* p_out, const int32_t* dir, int64_t n, int dim,
-                                   double eps, int n_steps, const FlowSchedule& sched,
-                                   int metric_kind, const double* minv, const mb200_model* model,
-                                   double* h_out, int32_t* status, int32_t* n_done,
-                                   cudaStream_t st, bool allow_dmma,
+// Launch functors of the leapfrog and the evaluation (eu_dispatch).  whole_vector: a user target
+// stages each chain's position and gradient in shared memory (user_target.cuh), 2 * 64 KP doubles
+// per warp more.
+struct LeapfrogLaunch {
+  static constexpr EuOp op = EuOp::Leapfrog;
+  const EuclidArgs& a;
+  const UserKernels* user;
+  bool k1_ok() const {
+    return a.allow_k1 && k1_serves(a.metric_kind, a.dim, a.eps, a.sched.step_sizes, a.n_steps,
+                                   a.sched.n_steps, a.m.target_id);
+  }
+  template <class Target>
+  int k1() const {
+    return k1_launch<Target>(a);
+  }
+  template <class Target, int L>
+  int warp() const {
+    constexpr int KP = EU_LAYOUTS[L].kp, CPW = EU_LAYOUTS[L].cpw;
+    return run(a.sched.gaussian ? leapfrog_generic_kernel<Target, KP, CPW, true>
+                                : leapfrog_generic_kernel<Target, KP, CPW, false>,
+               L, false);
+  }
+  int image(int l) const { return run(user->leapfrog[l], l, true); }
+  int run(LeapfrogKernel kern, int l, bool whole_vector) const {
+    constexpr int WARPS = 4;
+    const int kp = EU_LAYOUTS[l].kp, cpw = EU_LAYOUTS[l].cpw;
+    const size_t smem = (size_t)WARPS * (cpw + (whole_vector ? 2 : 0)) * 64 * kp * sizeof(double);
+    const int64_t groups = (a.n + cpw - 1) / cpw;
+    return eu_launch(kern, "leapfrog_generic_kernel", (groups + WARPS - 1) / WARPS, 16, WARPS * 32,
+                     smem, a.st, a.q_in, a.p_in, a.q_out, a.p_out, a.dir, a.n, a.dim, a.eps,
+                     a.n_steps, a.sched, a.metric_kind, a.minv, a.m, a.h_out, a.status, a.n_done);
+  }
+};
+
+struct EvalLaunch {
+  static constexpr EuOp op = EuOp::Eval;
+  const double *q, *p;
+  int64_t n;
+  int dim;
+  int metric_kind;
+  const double* minv;
+  ModelArgs m;
+  double *nld, *grad, *vel, *kin;
+  cudaStream_t st;
+  const UserKernels* user;
+  template <class Target, int L>
+  int warp() const {
+    return run(euclidean_eval_kernel<Target, EU_LAYOUTS[L].kp>, L, false);
+  }
+  int image(int l) const { return run(user->eval[l], l, true); }
+  int run(EvalKernel kern, int l, bool whole_vector) const {
+    constexpr int WARPS = 4;
+    const size_t smem = (size_t)WARPS * (whole_vector ? 3 : 1) * 64 * EU_LAYOUTS[l].kp * sizeof(double);
+    return eu_launch(kern, "euclidean_eval_kernel", (n + WARPS - 1) / WARPS, 16, WARPS * 32, smem,
+                     st, q, p, n, dim, metric_kind, minv, m, nld, grad, vel, kin);
+  }
+};
+
+// mb200_leapfrog_euclidean (allow_k1), _generic, _user (user != NULL) and
+// mb200_leapfrog_gaussian_euclidean (a.sched.gaussian)
+static int leapfrog_euclidean_impl(EuclidArgs a, const mb200_model* model,
                                    const UserKernels* user = nullptr) {
-  if (n == 0 && dim >= 1 && n_steps >= 0) return 0;  // empty batch: nothing to do
-  if (!q_in || !p_in || !q_out || !p_out || !model)
+  if (a.n == 0 && a.dim >= 1 && a.n_steps >= 0) return 0;  // empty batch: nothing to do
+  if (!a.q_in || !a.p_in || !a.q_out || !a.p_out || !model)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n < 0 || dim < 1 || n_steps < 0) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
-  if (metric_kind != MB200_METRIC_IDENTITY && !minv)
-    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
-  if (n == 0) return 0;
-  const DeviceScope device_scope(q_in);
-  const ModelArgs m = to_args(model);
-  if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
-    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
-  if (allow_dmma && metric_kind == MB200_METRIC_DENSE && n_steps > 0) {
-    int rc = leapfrog_dmma_dispatch(q_in, p_in, q_out, p_out, dir, sched.step_sizes, n, dim, eps,
-                                    n_steps, minv, m, h_out, status, n_done, st);
-    if (rc == 0) return check_launch("leapfrog_dmma_kernel");
-    if (rc != MB200_ERR_UNSUPPORTED) return fail(rc, "leapfrog_dmma launch failed");
-  }
-#define MB200_ARGS                                                                         \
-  q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, sched, metric_kind, minv, m, h_out, \
-      status, n_done, st
-  if (user != nullptr) {
-    if (m.target_id != MB200_TARGET_USER)
-      return fail(MB200_ERR_INVALID_ARG, "user-target entry point needs target_id MB200_TARGET_USER");
-    const int l = generic_layout(dim);
-    if (l < 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported by user targets", dim);
-    return launch_generic(user->leapfrog[l], GENERIC_KP[l], GENERIC_CPW[l], true, MB200_ARGS);
-  }
-  switch (m.target_id) {
-    case MB200_TARGET_STD_GAUSSIAN:
-      return dispatch_generic_dim<StdGaussianTarget>(MB200_ARGS);
-    case MB200_TARGET_NEAL_FUNNEL:
-      return dispatch_generic_dim<NealFunnelTarget>(MB200_ARGS);
-    case MB200_TARGET_BANANA:
-      return dispatch_generic_dim<BananaTarget>(MB200_ARGS);
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Euclidean leapfrog",
-                  m.target_id);
-  }
-#undef MB200_ARGS
+  if (a.n < 0 || a.dim < 1 || a.n_steps < 0) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
+  if (const int rc = eu_check_metric(a.metric_kind, a.minv)) return rc;
+  const DeviceScope device_scope(a.q_in);
+  a.m = to_args(model);
+  return eu_dispatch(a.m, a.dim, a.metric_kind, LeapfrogLaunch{a, user});
 }
 
-// mb200_leapfrog_euclidean (allow_dmma) and mb200_leapfrog_euclidean_generic
 static int leapfrog_euclidean_entry(const double* q_in, const double* p_in, double* q_out,
                                     double* p_out, const int32_t* dir, int64_t n, int dim,
                                     double eps, const double* step_sizes, int n_steps,
@@ -262,63 +215,17 @@ static int leapfrog_euclidean_entry(const double* q_in, const double* p_in, doub
                                     const double* coefficients, int initial_h1_flow_step,
                                     int metric_kind, const double* minv, const mb200_model* model,
                                     double* h_out, int32_t* status, int32_t* n_done,
-                                    cudaStream_t st, bool allow_dmma,
+                                    cudaStream_t st, bool allow_k1,
                                     const UserKernels* user = nullptr) {
   FlowSchedule s;
   if (const int rc = make_schedule(s, n_flows, coefficients, initial_h1_flow_step)) return rc;
   s.step_sizes = step_sizes;
   s.n_steps = n_steps_pc;
-  // the tensor-core kernel runs the leapfrog schedule with one trajectory length; with per-chain
-  // step sizes it scales the momentum tile by eps_c
-  allow_dmma = allow_dmma && coefficients == nullptr && n_steps_pc == nullptr;
-  return leapfrog_euclidean_impl(q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, s,
-                                 metric_kind, minv, model, h_out, status, n_done, st, allow_dmma,
-                                 user);
-}
-
-// One launch of `kern`, a euclidean_eval_kernel<Target, KP> of the library or of a user-target
-// image (whole_vector: 2 * 64 KP more doubles of shared memory per warp, as in launch_generic).
-static int launch_eval(const void* kern, int kp, bool whole_vector, const double* q,
-                       const double* p, int64_t n, int dim, int metric_kind, const double* minv,
-                       const ModelArgs& m, double* nld, double* grad, double* vel, double* kin,
-                       cudaStream_t st) {
-  constexpr int WARPS = 4;
-  const size_t smem = (size_t)WARPS * (whole_vector ? 3 : 1) * 64 * kp * sizeof(double);
-  if (smem > 48 * 1024) {
-    cudaError_t e =
-        cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  }
-  int64_t blocks = (n + WARPS - 1) / WARPS;
-  const int64_t cap = (int64_t)num_sms() * 16;
-  if (blocks > cap) blocks = cap;
-  ModelArgs ma = m;
-  void* args[] = {&q, &p, &n, &dim, &metric_kind, &minv, &ma, &nld, &grad, &vel, &kin};
-  const cudaError_t e =
-      cudaLaunchKernel(kern, dim3((unsigned)blocks), dim3(WARPS * 32), args, smem, st);
-  if (e != cudaSuccess) {
-    cudaGetLastError();  // reported here: clear it from the runtime's error state
-    return fail(MB200_ERR_CUDA, "euclidean_eval_kernel: %s", cudaGetErrorString(e));
-  }
-  return check_launch("euclidean_eval_kernel");
-}
-
-template <class Target>
-static int dispatch_eval_dim(const double* q, const double* p, int64_t n, int dim,
-                             int metric_kind, const double* minv, const ModelArgs& m, double* nld,
-                             double* grad, double* vel, double* kin, cudaStream_t st) {
-#define MB200_EV(L)                                                                           \
-  return launch_eval((const void*)euclidean_eval_kernel<Target, GENERIC_KP[L]>, GENERIC_KP[L],  \
-                     false, q, p, n, dim, metric_kind, minv, m, nld, grad, vel, kin, st)
-  switch (generic_layout(dim)) {
-    case 0: MB200_EV(0);
-    case 1: MB200_EV(1);
-    case 2: MB200_EV(2);
-    case 3: MB200_EV(3);
-    case 4: MB200_EV(4);
-  }
-#undef MB200_EV
-  return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported", dim);
+  // K1 runs the leapfrog schedule only
+  return leapfrog_euclidean_impl({q_in, p_in, q_out, p_out, dir, n, dim, eps, n_steps, s,
+                                  metric_kind, minv, ModelArgs(), h_out, status, n_done, st,
+                                  allow_k1 && coefficients == nullptr},
+                                 model, user);
 }
 
 // mb200_euclidean_eval and mb200_euclidean_eval_user (user != NULL)
@@ -330,28 +237,12 @@ static int euclidean_eval_impl(const double* pos, const double* mom, int64_t n_c
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos || !mom || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
-  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
-    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
-  if (n_chains == 0) return 0;
+  if (const int rc = eu_check_metric(metric_kind, metric_inv)) return rc;
   const DeviceScope device_scope(pos);
   const ModelArgs m = to_args(model);
-#define MB200_ARGS pos, mom, n_chains, dim, metric_kind, metric_inv, m, nld_out, grad_out, vel_out, kin_out, st
-  if (user != nullptr) {
-    if (m.target_id != MB200_TARGET_USER)
-      return fail(MB200_ERR_INVALID_ARG, "user-target entry point needs target_id MB200_TARGET_USER");
-    const int l = generic_layout(dim);
-    if (l < 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported by user targets", dim);
-    return launch_eval(user->eval[l], GENERIC_KP[l], true, MB200_ARGS);
-  }
-  switch (m.target_id) {
-    case MB200_TARGET_STD_GAUSSIAN: return dispatch_eval_dim<StdGaussianTarget>(MB200_ARGS);
-    case MB200_TARGET_NEAL_FUNNEL: return dispatch_eval_dim<NealFunnelTarget>(MB200_ARGS);
-    case MB200_TARGET_BANANA: return dispatch_eval_dim<BananaTarget>(MB200_ARGS);
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Euclidean eval", m.target_id);
-  }
-#undef MB200_ARGS
+  return eu_dispatch(m, dim, metric_kind,
+                     EvalLaunch{pos, mom, n_chains, dim, metric_kind, metric_inv, m, nld_out,
+                                grad_out, vel_out, kin_out, st, user});
 }
 
 }  // namespace mb200
@@ -429,17 +320,18 @@ int mb200_leapfrog_gaussian_euclidean(const double* pos_in, const double* mom_in
   s.gaussian = 1;
   s.rot = rotation;
   s.step_sizes = step_sizes;
-  return leapfrog_euclidean_impl(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
-                                 n_steps, s, metric_kind, metric_inv, model, h_out, status, n_done,
-                                 (cudaStream_t)stream, false);
+  return leapfrog_euclidean_impl({pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
+                                  n_steps, s, metric_kind, metric_inv, ModelArgs(), h_out, status,
+                                  n_done, (cudaStream_t)stream, false},
+                                 model);
 }
 
 int mb200_user_target_load(const void* image, int64_t image_bytes, const char* const* names,
                            int32_t n_names, void** handle) {
   if (!image || image_bytes <= 0 || !names || !handle)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_names != 2 * N_GENERIC_LAYOUTS)
-    return fail(MB200_ERR_INVALID_ARG, "expected %d kernel names, got %d", 2 * N_GENERIC_LAYOUTS,
+  if (n_names != 2 * N_EU_LAYOUTS)
+    return fail(MB200_ERR_INVALID_ARG, "expected %d kernel names, got %d", 2 * N_EU_LAYOUTS,
                 n_names);
   UserKernels* u = new UserKernels();
   cudaError_t e = cudaLibraryLoadData(&u->lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0);
@@ -455,7 +347,10 @@ int mb200_user_target_load(const void* image, int64_t image_bytes, const char* c
       delete u;
       return fail(MB200_ERR_CUDA, "cudaLibraryGetKernel(%s): %s", names[i], cudaGetErrorString(e));
     }
-    (i < N_GENERIC_LAYOUTS ? u->leapfrog[i] : u->eval[i - N_GENERIC_LAYOUTS]) = (const void*)k;
+    if (i < N_EU_LAYOUTS)
+      u->leapfrog[i] = reinterpret_cast<LeapfrogKernel>(k);
+    else
+      u->eval[i - N_EU_LAYOUTS] = reinterpret_cast<EvalKernel>(k);
   }
   *handle = u;
   return 0;
@@ -539,10 +434,10 @@ int mb200_leapfrog_euclidean_host(const double* pos_in, const double* mom_in, do
   double* d_po = d_qo + nd;
   int32_t* d_status = (int32_t*)(d_po + nd);
   int32_t* d_dir = d_status + n_chains;
-  // chunk boundaries on the granularity of a CTA of the kernel that will run (64 chains for the
-  // tensor-core kernel, 16 for the general one), so that the chunks together launch no more CTAs
-  // than one launch over all chains would
-  const int64_t align = (metric_kind == MB200_METRIC_DENSE && dim <= 128) ? 64 : 16;
+  // chunk boundaries on the granularity of a CTA of the kernel that will run (64 chains for K1, 16
+  // for K1g), so that the chunks together launch no more CTAs than one launch over all chains would
+  const int64_t align =
+      k1_serves(metric_kind, dim, step_size, nullptr, n_steps, nullptr, model->target_id) ? 64 : 16;
   int64_t per = (n_chains + n_chunks - 1) / n_chunks;
   per = (per + align - 1) / align * align;
   if (is_pageable(pos_in) || is_pageable(mom_in) || is_pageable(pos_out) || is_pageable(mom_out)) {

@@ -8,94 +8,59 @@
 
 namespace mb200 {
 
-// Shared dense metric, dim <= 128: the chains of a CTA in lock-step, mat-vecs on the tensor pipe
-template <class Target, int KP, int GROUPS>
-static int launch_nuts_dmma(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                            int64_t n, int dim, double eps, const double* minv, const ModelArgs& m,
-                            const NutsArgs& a, double* ws, double* h_out, int32_t* n_step,
-                            double* av_accept, double* reject_prob, int32_t* depth,
-                            int32_t* diverging, int32_t* n_used, int32_t* dir_out,
-                            int32_t* status, cudaStream_t st) {
-  auto kern = nuts_dmma_kernel<Target, KP, GROUPS>;
-  constexpr int WARPS = 8 * GROUPS;
-  const size_t smem = NutsDmmaLayout<KP, GROUPS>::smem_bytes();
-  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, WARPS * 32, smem);
-  if (per_sm < 1) per_sm = 1;
-  int64_t blocks = (n + WARPS - 1) / WARPS;
-  const int64_t cap = (int64_t)num_sms() * per_sm;
-  if (blocks > cap) blocks = cap;
-  kern<<<(unsigned)blocks, WARPS * 32, smem, st>>>(q_in, p_in, q_out, p_out, n, dim, eps, minv, m,
-                                                    a, ws, h_out, n_step, av_accept, reject_prob,
-                                                    depth, diverging, n_used, dir_out, status);
-  return check_launch("nuts_dmma_kernel");
-}
+// Arguments and launches of fused Euclidean NUTS (eu_dispatch)
+struct NutsLaunch {
+  static constexpr EuOp op = EuOp::Nuts;
+  const double *q_in, *p_in;
+  double *q_out, *p_out;
+  int64_t n;
+  int dim;
+  double eps;
+  int metric_kind;
+  const double* minv;
+  ModelArgs m;
+  NutsArgs a;
+  double* ws;
+  double* h_out;
+  int32_t* n_step;
+  double *av_accept, *reject_prob;
+  int32_t *depth, *diverging, *n_used, *dir_out, *status;
+  cudaStream_t st;
 
-template <class Target, int KP>
-static int launch_nuts(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                       int64_t n, int dim, double eps, int metric_kind, const double* minv,
-                       const ModelArgs& m, const NutsArgs& a, double* ws, double* h_out,
-                       int32_t* n_step, double* av_accept, double* reject_prob, int32_t* depth,
-                       int32_t* diverging, int32_t* n_used, int32_t* dir_out, int32_t* status,
-                       cudaStream_t st) {
-  if constexpr (KP <= 2) {
-    // shared dense metric, dim <= 128: groups of 8 chains in lock-step, mat-vecs on the tensor
-    // pipe.  Measured on C1 (depth 6; free-running nuts_euclidean_kernel: 95 M leapfrog steps/s):
-    // one group per CTA 205 M, two groups 172 M (register spills at the 128-register budget and
-    // a workspace working set beyond L2), 16 chains in one lock-step 168 M; at dim = 64 (depth 8)
-    // two groups 377 M, one group 300 M, free-running 215 M.
-    if (metric_kind == MB200_METRIC_DENSE && dim >= 8)
-      return launch_nuts_dmma<Target, KP, (KP == 1 ? 2 : 1)>(
-          q_in, p_in, q_out, p_out, n, dim, eps, minv, m, a, ws, h_out, n_step, av_accept,
-          reject_prob, depth, diverging, n_used, dir_out, status, st);
+  // Shared dense metric, dim <= 128: groups of 8 chains in lock-step, mat-vecs on the tensor pipe.
+  // Measured on C1 (depth 6; free-running nuts_euclidean_kernel: 95 M leapfrog steps/s): one
+  // group per CTA 205 M, two groups 172 M (register spills at the 128-register budget and a
+  // workspace working set beyond L2), 16 chains in one lock-step 168 M; at dim = 64 (depth 8) two
+  // groups 377 M, one group 300 M, free-running 215 M.
+  template <class Target, int L>
+  int dmma() const {
+    constexpr int KP = EU_LAYOUTS[L].kp, GROUPS = KP == 1 ? 2 : 1, WARPS = 8 * GROUPS;
+    return eu_launch(nuts_dmma_kernel<Target, KP, GROUPS>, "nuts_dmma_kernel",
+                     (n + WARPS - 1) / WARPS, 0, WARPS * 32, NutsDmmaLayout<KP, GROUPS>::smem_bytes(),
+                     st, q_in, p_in, q_out, p_out, n, dim, eps, minv, m, a, ws, h_out, n_step,
+                     av_accept, reject_prob, depth, diverging, n_used, dir_out, status);
   }
-  auto kern = nuts_euclidean_kernel<Target, KP>;
-  NutsArgs args = a;
-  // dense metric that fits in shared memory next to the staging rows: the warps of a CTA share it
-  // (12 warps for 64 < dim <= 128, where one CTA per SM fits; 8 otherwise -- measured)
-  const size_t metric_bytes = (size_t)dim * dim * sizeof(double);
-  const int staged_warps = KP == 2 ? 12 : 8;
-  args.stage_metric = metric_kind == MB200_METRIC_DENSE &&
-                      metric_bytes + staged_warps * 64 * KP * sizeof(double) <= 200 * 1024;
-  const int warps = args.stage_metric ? staged_warps : 4;
-  const size_t smem = (size_t)warps * 64 * KP * sizeof(double) + (args.stage_metric ? metric_bytes : 0);
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  }
-  int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, warps * 32, smem);
-  if (per_sm < 1) per_sm = 1;
-  int64_t blocks = (n + warps - 1) / warps;
-  const int64_t cap = (int64_t)num_sms() * per_sm;
-  if (blocks > cap) blocks = cap;
-  kern<<<(unsigned)blocks, warps * 32, smem, st>>>(
-      q_in, p_in, q_out, p_out, n, dim, eps, metric_kind, minv, m, args, ws, h_out, n_step,
-      av_accept, reject_prob, depth, diverging, n_used, dir_out, status);
-  return check_launch("nuts_euclidean_kernel");
-}
 
-template <class Target>
-static int dispatch_nuts_dim(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                             int64_t n, int dim, double eps, int metric_kind, const double* minv,
-                             const ModelArgs& m, const NutsArgs& a, double* ws, double* h_out,
-                             int32_t* n_step, double* av_accept, double* reject_prob,
-                             int32_t* depth, int32_t* diverging, int32_t* n_used,
-                             int32_t* dir_out, int32_t* status, cudaStream_t st) {
-#define MB200_NUTS(KP)                                                                         \
-  return launch_nuts<Target, KP>(q_in, p_in, q_out, p_out, n, dim, eps, metric_kind, minv, m, a, \
-                                 ws, h_out, n_step, av_accept, reject_prob, depth, diverging,  \
-                                 n_used, dir_out, status, st)
-  if (dim <= 64) MB200_NUTS(1);
-  if (dim <= 128) MB200_NUTS(2);
-  if (dim <= 256) MB200_NUTS(4);
-  if (dim <= 512) MB200_NUTS(8);
-  if (dim <= 1024) MB200_NUTS(16);
-#undef MB200_NUTS
-  return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported", dim);
-}
+  // Free-running: one warp per chain
+  template <class Target, int L>
+  int warp() const {
+    constexpr int KP = EU_LAYOUTS[L].kp;
+    NutsArgs args = a;
+    // dense metric that fits in shared memory next to the staging rows: the warps of a CTA share
+    // it (12 warps for 64 < dim <= 128, where one CTA per SM fits; 8 otherwise -- measured)
+    const size_t metric_bytes = (size_t)dim * dim * sizeof(double);
+    const int staged_warps = KP == 2 ? 12 : 8;
+    args.stage_metric = metric_kind == MB200_METRIC_DENSE &&
+                        metric_bytes + staged_warps * 64 * KP * sizeof(double) <= 200 * 1024;
+    const int warps = args.stage_metric ? staged_warps : 4;
+    const size_t smem =
+        (size_t)warps * 64 * KP * sizeof(double) + (args.stage_metric ? metric_bytes : 0);
+    return eu_launch(nuts_euclidean_kernel<Target, KP>, "nuts_euclidean_kernel",
+                     (n + warps - 1) / warps, 0, warps * 32, smem, st, q_in, p_in, q_out, p_out, n,
+                     dim, eps, metric_kind, minv, m, args, ws, h_out, n_step, av_accept,
+                     reject_prob, depth, diverging, n_used, dir_out, status);
+  }
+};
 
 }  // namespace mb200
 
@@ -159,18 +124,13 @@ int mb200_nuts_euclidean(const double* pos_in, const double* mom_in, double* pos
   if (n_chains < 0 || dim < 1 || n_uniforms < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
   if (max_tree_depth < 1 || max_tree_depth > NUTS_MAX_DEPTH)
     return fail(MB200_ERR_INVALID_ARG, "max_tree_depth must be in [1, %d]", NUTS_MAX_DEPTH);
-  if (metric_kind < 0 || metric_kind > 2) return fail(MB200_ERR_INVALID_ARG, "bad metric_kind");
-  if (metric_kind != MB200_METRIC_IDENTITY && !metric_inv)
-    return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
+  if (const int rc = eu_check_metric(metric_kind, metric_inv)) return rc;
+  // need < 0: dim > 1024, which the dispatch reports
   const int64_t need = mb200_nuts_workspace_bytes(n_chains, dim, max_tree_depth);
-  if (need < 0) return fail(MB200_ERR_UNSUPPORTED, "dim %d > 1024 not supported", dim);
-  if (workspace_bytes < need)
+  if (need >= 0 && workspace_bytes < need)
     return fail(MB200_ERR_INVALID_ARG, "workspace too small: %lld < %lld bytes",
                 (long long)workspace_bytes, (long long)need);
   const DeviceScope device_scope(pos_in);
-  const ModelArgs m = to_args(model);
-  if (m.target_id == MB200_TARGET_BANANA && (dim & 1))
-    return fail(MB200_ERR_INVALID_ARG, "banana target needs even dim");
   NutsArgs a;
   a.max_depth = max_tree_depth;
   a.max_delta_h = max_delta_h;
@@ -181,20 +141,12 @@ int mb200_nuts_euclidean(const double* pos_in, const double* mom_in, double* pos
   a.n_uniforms = n_uniforms;
   a.step_sizes = step_sizes;
   a.stage_metric = 0;
-  cudaStream_t st = (cudaStream_t)stream;
-#define MB200_ARGS                                                                             \
-  pos_in, mom_in, pos_out, mom_out, n_chains, dim, step_size, metric_kind, metric_inv, m, a,   \
-      (double*)workspace, h_out, n_step, av_metrop_accept_prob, reject_prob, tree_depth,       \
-      diverging, n_uniforms_used, dir_out, status, st
-  switch (m.target_id) {
-    case MB200_TARGET_STD_GAUSSIAN: return dispatch_nuts_dim<StdGaussianTarget>(MB200_ARGS);
-    case MB200_TARGET_NEAL_FUNNEL: return dispatch_nuts_dim<NealFunnelTarget>(MB200_ARGS);
-    case MB200_TARGET_BANANA: return dispatch_nuts_dim<BananaTarget>(MB200_ARGS);
-    default:
-      return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Euclidean NUTS",
-                  m.target_id);
-  }
-#undef MB200_ARGS
+  const ModelArgs m = to_args(model);
+  return eu_dispatch(m, dim, metric_kind,
+                     NutsLaunch{pos_in, mom_in, pos_out, mom_out, n_chains, dim, step_size,
+                                metric_kind, metric_inv, m, a, (double*)workspace, h_out, n_step,
+                                av_metrop_accept_prob, reject_prob, tree_depth, diverging,
+                                n_uniforms_used, dir_out, status, (cudaStream_t)stream});
 }
 
 // ---------------------------------------------------------------- generic dynamic transitions
@@ -228,15 +180,6 @@ unsigned gen_blocks(int64_t n) {
 
 }  // namespace
 
-#define MB200_KP_DISPATCH(CALL)                 \
-  do {                                          \
-    if (dim <= 64) { CALL(1); }                 \
-    else if (dim <= 128) { CALL(2); }           \
-    else if (dim <= 256) { CALL(4); }           \
-    else if (dim <= 512) { CALL(8); }           \
-    else { CALL(16); }                          \
-  } while (0)
-
 int64_t mb200_nuts_generic_state_bytes(int64_t n_chains) {
   return n_chains < 0 ? -1 : n_chains * (int64_t)sizeof(NutsGenState);
 }
@@ -255,11 +198,12 @@ int mb200_nuts_generic_begin(const double* pos, const double* mom, const double*
   const DeviceScope device_scope(pos);
   const NutsGenArgs a = gen_args(options);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(KP)                                                                              \
-  nuts_generic_begin_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(                        \
-      pos, mom, vel, h, n_chains, dim, a, (double*)workspace, (NutsGenState*)chain_state)
-  MB200_KP_DISPATCH(CALL);
-#undef CALL
+  with_layout(dim, [&](auto lay) {
+    constexpr int KP = EU_LAYOUTS[decltype(lay)::value].kp;
+    nuts_generic_begin_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(
+        pos, mom, vel, h, n_chains, dim, a, (double*)workspace, (NutsGenState*)chain_state);
+    return 0;
+  });
   return check_launch("nuts_generic_begin_kernel");
 }
 
@@ -274,12 +218,13 @@ int mb200_nuts_generic_start(int64_t n_chains, int32_t dim, int32_t depth,
   const DeviceScope device_scope(pos_edge);
   const NutsGenArgs a = gen_args(options);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(KP)                                                                           \
-  nuts_generic_start_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(                     \
-      n_chains, dim, depth, a, (double*)workspace, (NutsGenState*)chain_state, pos_edge,   \
-      mom_edge, dir_out, active)
-  MB200_KP_DISPATCH(CALL);
-#undef CALL
+  with_layout(dim, [&](auto lay) {
+    constexpr int KP = EU_LAYOUTS[decltype(lay)::value].kp;
+    nuts_generic_start_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(
+        n_chains, dim, depth, a, (double*)workspace, (NutsGenState*)chain_state, pos_edge,
+        mom_edge, dir_out, active);
+    return 0;
+  });
   return check_launch("nuts_generic_start_kernel");
 }
 
@@ -294,12 +239,13 @@ int mb200_nuts_generic_leaf(const double* pos, const double* mom, const double* 
   const DeviceScope device_scope(pos);
   const NutsGenArgs a = gen_args(options);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(KP)                                                                              \
-  nuts_generic_leaf_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(                         \
-      pos, mom, vel, h, status, n_chains, dim, k, n_leaves, a, (double*)workspace,            \
-      (NutsGenState*)chain_state, active)
-  MB200_KP_DISPATCH(CALL);
-#undef CALL
+  with_layout(dim, [&](auto lay) {
+    constexpr int KP = EU_LAYOUTS[decltype(lay)::value].kp;
+    nuts_generic_leaf_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(
+        pos, mom, vel, h, status, n_chains, dim, k, n_leaves, a, (double*)workspace,
+        (NutsGenState*)chain_state, active);
+    return 0;
+  });
   return check_launch("nuts_generic_leaf_kernel");
 }
 
@@ -311,11 +257,12 @@ int mb200_nuts_generic_finish(int64_t n_chains, int32_t dim, int32_t depth,
   const DeviceScope device_scope(workspace);
   const NutsGenArgs a = gen_args(options);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(KP)                                                                  \
-  nuts_generic_finish_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(           \
-      n_chains, dim, depth, a, (double*)workspace, (NutsGenState*)chain_state)
-  MB200_KP_DISPATCH(CALL);
-#undef CALL
+  with_layout(dim, [&](auto lay) {
+    constexpr int KP = EU_LAYOUTS[decltype(lay)::value].kp;
+    nuts_generic_finish_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(
+        n_chains, dim, depth, a, (double*)workspace, (NutsGenState*)chain_state);
+    return 0;
+  });
   return check_launch("nuts_generic_finish_kernel");
 }
 
@@ -332,13 +279,14 @@ int mb200_nuts_generic_end(int64_t n_chains, int32_t dim, const mb200_nuts_optio
   const DeviceScope device_scope(pos_out);
   const NutsGenArgs a = gen_args(options);
   cudaStream_t st = (cudaStream_t)stream;
-#define CALL(KP)                                                                               \
-  nuts_generic_end_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(                           \
-      n_chains, dim, a, (const double*)workspace, (const NutsGenState*)chain_state, pos_out,    \
-      mom_out, h_out, n_step, av_metrop_accept_prob, reject_prob, tree_depth, flags_out,       \
-      n_uniforms_used, dir_out)
-  MB200_KP_DISPATCH(CALL);
-#undef CALL
+  with_layout(dim, [&](auto lay) {
+    constexpr int KP = EU_LAYOUTS[decltype(lay)::value].kp;
+    nuts_generic_end_kernel<KP><<<gen_blocks(n_chains), 128, 0, st>>>(
+        n_chains, dim, a, (const double*)workspace, (const NutsGenState*)chain_state, pos_out,
+        mom_out, h_out, n_step, av_metrop_accept_prob, reject_prob, tree_depth, flags_out,
+        n_uniforms_used, dir_out);
+    return 0;
+  });
   return check_launch("nuts_generic_end_kernel");
 }
 

@@ -633,76 +633,4 @@ __global__ void __launch_bounds__(DMMA_THREADS, 1)
   }
 }
 
-template <class Target, int DP, bool PC>
-static int launch_dmma(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                       const int32_t* dir, const double* step_sizes, int64_t n, int dim,
-                       double eps, int n_steps,
-                       const double* minv, const ModelArgs& m, double* h_out, int32_t* status,
-                       int32_t* n_done, cudaStream_t st, int sms) {
-  auto kern = leapfrog_dmma_kernel<Target, DP, PC>;
-  const size_t smem = sizeof(DmmaSmem<DP>);
-  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
-      cudaSuccess)
-    return MB200_ERR_CUDA;
-  const int64_t total_tiles = (n + 7) / 8;
-  int64_t tpc = (total_tiles + sms - 1) / sms;  // tiles per CTA and pass
-  if (tpc > DMMA_TILES_PER_CTA) tpc = DMMA_TILES_PER_CTA;
-  int64_t blocks = (total_tiles + tpc - 1) / tpc;
-  if (blocks > sms) blocks = sms;
-  auto al16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-  const int even = (dim & 1) == 0;
-  const int vec2 = even && al16(q_in) && al16(p_in) && al16(q_out) && al16(p_out);
-  const int tma_rows = even && al16(minv);  // persistent: CTAs loop over passes of tpc tiles
-  kern<<<(unsigned)blocks, DMMA_THREADS, smem, st>>>(q_in, p_in, q_out, p_out, dir, step_sizes, n,
-                                                     dim, PC ? 1.0 : eps, n_steps, minv, m, h_out,
-                                                     status, n_done, (int)tpc, vec2, tma_rows);
-  return 0;
-}
-
-template <class Target>
-static int dispatch_dmma_dim(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                             const int32_t* dir, const double* step_sizes, int64_t n, int dim,
-                             double eps, int n_steps,
-                             const double* minv, const ModelArgs& m, double* h_out,
-                             int32_t* status, int32_t* n_done, cudaStream_t st, int sms) {
-#define MB200_DM(DP)                                                                        \
-  return step_sizes != nullptr                                                              \
-             ? launch_dmma<Target, DP, true>(q_in, p_in, q_out, p_out, dir, step_sizes, n,  \
-                                             dim, eps, n_steps, minv, m, h_out, status,     \
-                                             n_done, st, sms)                               \
-             : launch_dmma<Target, DP, false>(q_in, p_in, q_out, p_out, dir, nullptr, n,    \
-                                              dim, eps, n_steps, minv, m, h_out, status,    \
-                                              n_done, st, sms)
-  if (dim <= 32) MB200_DM(32);
-  if (dim <= 64) MB200_DM(64);
-  if (dim <= 96) MB200_DM(96);
-  MB200_DM(128);
-#undef MB200_DM
-}
-
-// Returns MB200_ERR_UNSUPPORTED when the shape is outside this kernel's domain (the caller
-// then uses the general-dimension kernel).
-int leapfrog_dmma_dispatch(const double* q_in, const double* p_in, double* q_out, double* p_out,
-                           const int32_t* dir, const double* step_sizes, int64_t n, int dim,
-                           double eps, int n_steps,
-                           const double* minv, const ModelArgs& m, double* h_out, int32_t* status,
-                           int32_t* n_done, cudaStream_t st) {
-  if (dim > 128 || dim < 8) return MB200_ERR_UNSUPPORTED;
-  if (step_sizes == nullptr && (!(eps != 0.0) || !isfinite(eps)))
-    return MB200_ERR_UNSUPPORTED;  // eps*A formulation
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-#define MB200_ARGS                                                                             \
-  q_in, p_in, q_out, p_out, dir, step_sizes, n, dim, eps, n_steps, minv, m, h_out, status, n_done, \
-      st, sms
-  switch (m.target_id) {
-    case MB200_TARGET_STD_GAUSSIAN: return dispatch_dmma_dim<StdGaussianTarget>(MB200_ARGS);
-    case MB200_TARGET_NEAL_FUNNEL: return dispatch_dmma_dim<NealFunnelTarget>(MB200_ARGS);
-    case MB200_TARGET_BANANA: return dispatch_dmma_dim<BananaTarget>(MB200_ARGS);
-    default: return MB200_ERR_UNSUPPORTED;
-  }
-#undef MB200_ARGS
-}
-
 }  // namespace mb200

@@ -29,7 +29,8 @@ ARCH = "sm_90a"
 # -default-device: the C prototypes of include/mici_b200.h become (unused) device declarations.
 OPTIONS = ("-arch=" + ARCH, "-std=c++17", "-fmad=false", "-default-device")
 
-# (KP, CPW) of the general-dimension kernel, in the kernel-table order of mb200_user_target_load
+# (KP, CPW) of the general-dimension kernel, in the kernel-table order of mb200_user_target_load:
+# the order of EU_LAYOUTS in csrc/api_common.cuh, which this list must keep
 LAYOUTS = ((1, 4), (2, 4), (4, 2), (8, 1), (16, 1))
 NAME_EXPRESSIONS = tuple(
     [f"&mb200::leapfrog_generic_kernel<mb200::UserTarget, {kp}, {cpw}, false>" for kp, cpw in LAYOUTS]

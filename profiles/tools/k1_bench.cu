@@ -40,7 +40,8 @@ __device__ unsigned long long g_gt[2][8];
     }                                                                                  \
   } while (0)
 #endif
-#include "../../mici_b200/csrc/leapfrog_dmma.cuh"
+// K1's host launcher (k1_launch) and its kernel, as the library builds them
+#include "../../mici_b200/csrc/api_dmma.cu"
 
 using namespace mb200;
 
@@ -81,11 +82,14 @@ int main(int argc, char** argv) {
     float best = 1e30f;
     for (int rep = 0; rep < 6; ++rep) {
       cudaEventRecord(e0);
-      int rc = leapfrog_dmma_dispatch(dq, dp, dqo, dpo, nullptr, nullptr, n, dim, 0.01, steps, dm, m, with_h ? dh : nullptr, dst,
-                                      dnd, 0);
+      EuclidArgs a{};
+      a.q_in = dq, a.p_in = dp, a.q_out = dqo, a.p_out = dpo, a.n = n, a.dim = dim, a.eps = 0.01;
+      a.n_steps = steps, a.minv = dm, a.m = m, a.h_out = with_h ? dh : nullptr, a.status = dst;
+      a.n_done = dnd;
+      int rc = k1_launch<NealFunnelTarget>(a);
       cudaEventRecord(e1);
       cudaEventSynchronize(e1);
-      if (rc != 0) { printf("dispatch rc=%d\n", rc); return 1; }
+      if (rc != 0) { printf("k1_launch rc=%d: %s\n", rc, g_err); return 1; }
       float ms;
       cudaEventElapsedTime(&ms, e0, e1);
       if (rep > 0 && ms < best) best = ms;

@@ -319,3 +319,280 @@ def test_constrained_projection_routing(lib, gaussian):
                 if err:
                     failures.append(f"target {target} nc {n_constr} dim {dim} metric {metric_kind}: {err}")
     assert not failures, f"{len(failures)} cases:\n" + "\n".join(failures[:40])
+
+
+# --- Euclidean entry points -----------------------------------------------------------------------
+#
+# A routed Euclidean call fails at its first CUDA call with "<kernel>: <CUDA error>", so the message
+# names the kernel that would have run: the tensor-core leapfrog K1 (leapfrog_dmma_kernel), the
+# general-dimension leapfrog K1g (leapfrog_generic_kernel), the evaluation kernel, and fused NUTS in
+# lock-step on the tensor pipe (nuts_dmma_kernel) or free-running (nuts_euclidean_kernel).
+
+USER = 64
+UNKNOWN_TARGET = 9
+EUCLID_TARGETS = tuple(range(8)) + (UNKNOWN_TARGET,)
+EUCLID_DIMS = (1, 2, 7, 8, 64, 65, 128, 129, 1024, 1025)
+# (per-chain step sizes, per-chain lengths, coefficient schedule) of a leapfrog call
+SCHEDULES = {
+    "shared_eps": (False, False, False),
+    "per_chain_eps": (True, False, False),
+    "per_chain_lengths": (False, True, False),
+    "coefficients": (False, False, True),
+}
+COEFS = np.array([0.25, 0.5, 0.5, 0.5, 0.25])
+# a user-target handle whose kernel table is empty: calls that reach a launch fail there
+FAKE_IMAGE = np.zeros(16, dtype=np.uint64)
+
+
+def euclid_model_expected(target, dim, metric_kind, minv, user):
+    """The model checks every Euclidean operation applies, in order; None when the model passes."""
+    if metric_kind > 2:
+        return (INVALID, "bad metric_kind")
+    if metric_kind != 0 and minv is None:
+        return (INVALID, "metric_inv is NULL")
+    if target == BANANA and dim % 2:
+        return (INVALID, "banana target needs even dim")
+    if user and target != USER:
+        return (INVALID, "user-target entry point needs target_id MB200_TARGET_USER")
+    if not user and target not in (STD, FUNNEL, BANANA):
+        return (UNSUPPORTED, f"target {target} not available")
+    if dim > 1024:
+        return (UNSUPPORTED, f"dim {dim} > 1024 not supported")
+    return None
+
+
+def k1_serves(target, dim, metric_kind, eps, per_chain_eps, n_steps, schedule):
+    _, per_chain_lengths, coefficients = SCHEDULES[schedule]
+    return (metric_kind == 2 and n_steps > 0 and 8 <= dim <= 128 and not per_chain_lengths
+            and not coefficients and (per_chain_eps or (eps != 0 and np.isfinite(eps)))
+            and target in (STD, FUNNEL, BANANA))
+
+
+def leapfrog_call(lib, entry, m, dim, metric_kind, minv, schedule, eps=0.1, n_steps=1, user=None):
+    per_chain_eps, per_chain_lengths, coefficients = SCHEDULES[schedule]
+    args = [PTR, PTR, PTR, PTR, None, 4, dim, eps, PTR if per_chain_eps else None, n_steps,
+            PTR if per_chain_lengths else None, len(COEFS) if coefficients else 0,
+            COEFS.ctypes.data if coefficients else None, 1, metric_kind, minv, ctypes.byref(m),
+            PTR, PTR, PTR, None]
+    if entry == "user":
+        return call(lib, "mb200_leapfrog_euclidean_user", *args, user)
+    return call(lib, f"mb200_leapfrog_euclidean{'_generic' if entry == 'generic' else ''}", *args)
+
+
+@pytest.mark.parametrize("entry", ("leapfrog", "generic", "user"))
+def test_euclidean_leapfrog_routing(lib, entry):
+    user = entry == "user"
+    failures = []
+    for target in EUCLID_TARGETS + ((USER,) if user else ()):
+        for dim in EUCLID_DIMS:
+            for metric_kind in (0, 1, 2, 3):
+                for minv in (PTR, None):
+                    for schedule in SCHEDULES:
+                        m = model(target, tp=(1.0,))
+                        got = leapfrog_call(lib, entry, m, dim, metric_kind, minv, schedule,
+                                            user=FAKE_IMAGE.ctypes.data if user else None)
+                        want = euclid_model_expected(target, dim, metric_kind, minv, user)
+                        if want is None:
+                            k1 = entry == "leapfrog" and k1_serves(
+                                target, dim, metric_kind, 0.1, SCHEDULES[schedule][0], 1, schedule)
+                            want = (CUDA, "leapfrog_dmma_kernel: " if k1 else "leapfrog_generic_kernel: ")
+                        err = check(got, want)
+                        if err:
+                            failures.append(f"target {target} dim {dim} metric {metric_kind} "
+                                            f"minv {minv is not None} {schedule}: {err}")
+    assert not failures, f"{len(failures)} cases:\n" + "\n".join(failures[:40])
+
+
+def test_euclidean_leapfrog_k1_needs_a_usable_step_size(lib):
+    m = model(FUNNEL)
+    for eps, n_steps in ((0.0, 1), (float("nan"), 1), (float("inf"), 1), (0.1, 0)):
+        got = leapfrog_call(lib, "leapfrog", m, 64, 2, PTR, "shared_eps", eps=eps, n_steps=n_steps)
+        assert check(got, (CUDA, "leapfrog_generic_kernel: ")) is None, (eps, n_steps, got)
+        # per-chain step sizes: the scalar is not used
+        got = leapfrog_call(lib, "leapfrog", m, 64, 2, PTR, "per_chain_eps", eps=eps, n_steps=n_steps)
+        want = "leapfrog_dmma_kernel: " if n_steps > 0 else "leapfrog_generic_kernel: "
+        assert check(got, (CUDA, want)) is None, (eps, n_steps, got)
+
+
+def test_euclidean_bad_arguments_are_rejected(lib):
+    m = model(STD)
+    args = [PTR, PTR, PTR, PTR, None, 4, 8, 0.1, None, 1, None, 0, None, 1, 0, None,
+            ctypes.byref(m), PTR, PTR, PTR, None]
+    name = "mb200_leapfrog_euclidean"
+    assert check(call(lib, name, *args[:3], None, *args[4:]), (INVALID, "null pointer")) is None
+    assert check(call(lib, name, *args[:6], 0, *args[7:]), (INVALID, "bad sizes")) is None
+    assert check(call(lib, name, *args[:9], -1, *args[10:]), (INVALID, "bad sizes")) is None
+    assert check(call(lib, name, *args[:11], 2, COEFS.ctypes.data, *args[13:]),
+                 (INVALID, "n_flows must be odd")) is None
+    # an empty batch returns before any other check
+    assert call(lib, name, *args[:5], 0, *args[6:])[0] == 0
+    assert call(lib, name, None, *args[1:5], 0, *args[6:])[0] == 0
+    assert call(lib, "mb200_euclidean_eval", None, PTR, 0, 8, 0, None, ctypes.byref(m), PTR, PTR,
+                PTR, PTR, None)[0] == 0
+
+
+@pytest.mark.parametrize("user", (False, True))
+def test_euclidean_hamiltonian_routing(lib, user):
+    failures = []
+    for target in EUCLID_TARGETS + ((USER,) if user else ()):
+        for dim in EUCLID_DIMS:
+            for metric_kind in (0, 1, 2, 3):
+                for minv in (PTR, None):
+                    m = model(target, tp=(1.0,))
+                    args = [PTR, PTR, 4, dim, metric_kind, minv, ctypes.byref(m)]
+                    name = "mb200_hamiltonian_euclidean" + ("_user" if user else "")
+                    tail = [None, FAKE_IMAGE.ctypes.data] if user else [None]
+                    want = euclid_model_expected(target, dim, metric_kind, minv, user) or (
+                        CUDA, "leapfrog_generic_kernel: ")
+                    for h_out in (PTR, None):
+                        got = call(lib, name, *args, h_out, *tail)
+                        err = check(got, want if h_out else (INVALID, "h_out is NULL"))
+                        if err:
+                            failures.append(f"target {target} dim {dim} metric {metric_kind} "
+                                            f"minv {minv is not None} h_out {h_out}: {err}")
+    assert not failures, f"{len(failures)} cases:\n" + "\n".join(failures[:40])
+
+
+@pytest.mark.parametrize("user", (False, True))
+def test_euclidean_eval_routing(lib, user):
+    failures = []
+    for target in EUCLID_TARGETS + ((USER,) if user else ()):
+        for dim in EUCLID_DIMS:
+            for metric_kind in (0, 1, 2, 3):
+                for minv in (PTR, None):
+                    m = model(target, tp=(1.0,))
+                    args = [PTR, PTR, 4, dim, metric_kind, minv, ctypes.byref(m), PTR, PTR, PTR, PTR,
+                            None]
+                    got = (call(lib, "mb200_euclidean_eval_user", *args, FAKE_IMAGE.ctypes.data)
+                           if user else call(lib, "mb200_euclidean_eval", *args))
+                    want = euclid_model_expected(target, dim, metric_kind, minv, user) or (
+                        CUDA, "euclidean_eval_kernel: ")
+                    err = check(got, want)
+                    if err:
+                        failures.append(f"target {target} dim {dim} metric {metric_kind} "
+                                        f"minv {minv is not None}: {err}")
+    assert not failures, f"{len(failures)} cases:\n" + "\n".join(failures[:40])
+
+
+def test_euclidean_gaussian_leapfrog_routing(lib):
+    failures = []
+    for target in EUCLID_TARGETS:
+        for dim in EUCLID_DIMS:
+            for metric_kind in (0, 1, 2, 3):
+                for minv in (PTR, None):
+                    for rotation in (PTR, None):
+                        for per_chain_eps in (False, True):
+                            m = model(target, tp=(1.0,))
+                            got = call(lib, "mb200_leapfrog_gaussian_euclidean", PTR, PTR, PTR, PTR,
+                                       None, 4, dim, 0.1, PTR if per_chain_eps else None, 1, 0, None,
+                                       1, metric_kind, minv, rotation, ctypes.byref(m), PTR, PTR, PTR,
+                                       None)
+                            if metric_kind != 0 and rotation is None:
+                                want = (INVALID, "rotation is NULL")
+                            elif metric_kind == 2 and per_chain_eps:
+                                want = (UNSUPPORTED, "per-chain step sizes need per-chain rotation")
+                            else:
+                                want = euclid_model_expected(target, dim, metric_kind, minv, False) or (
+                                    CUDA, "leapfrog_generic_kernel: ")
+                            err = check(got, want)
+                            if err:
+                                failures.append(f"target {target} dim {dim} metric {metric_kind} "
+                                                f"minv {minv is not None} rotation {rotation} "
+                                                f"per-chain eps {per_chain_eps}: {err}")
+    assert not failures, f"{len(failures)} cases:\n" + "\n".join(failures[:40])
+
+
+@pytest.mark.parametrize("name", ("mb200_leapfrog_euclidean_user", "mb200_hamiltonian_euclidean_user",
+                                  "mb200_euclidean_eval_user"))
+def test_euclidean_null_user_target_is_rejected(lib, name):
+    m = model(USER)
+    if name == "mb200_leapfrog_euclidean_user":
+        got = leapfrog_call(lib, "user", m, 8, 0, None, "shared_eps", user=None)
+    elif name == "mb200_hamiltonian_euclidean_user":
+        got = call(lib, name, PTR, PTR, 4, 8, 0, None, ctypes.byref(m), PTR, None, None)
+    else:
+        got = call(lib, name, PTR, PTR, 4, 8, 0, None, ctypes.byref(m), PTR, PTR, PTR, PTR, None, None)
+    assert check(got, (INVALID, "user_target is NULL")) is None, got
+
+
+def nuts_call(lib, m, dim, metric_kind, minv, workspace_bytes=1 << 40, depth=6, uniforms=PTR):
+    return call(lib, "mb200_nuts_euclidean", PTR, PTR, PTR, PTR, 4, dim, 0.1, None, metric_kind,
+                minv, ctypes.byref(m), 0, 0, 0, depth, 1000.0, uniforms, 8, PTR, workspace_bytes,
+                PTR, PTR, PTR, PTR, PTR, PTR, PTR, PTR, PTR, None)
+
+
+def test_euclidean_nuts_routing(lib):
+    failures = []
+    for target in EUCLID_TARGETS:
+        for dim in EUCLID_DIMS:
+            for metric_kind in (0, 1, 2, 3):
+                for minv in (PTR, None):
+                    m = model(target, tp=(1.0,))
+                    want = euclid_model_expected(target, dim, metric_kind, minv, False)
+                    if want is None:
+                        dmma = metric_kind == 2 and 8 <= dim <= 128
+                        want = (CUDA, "nuts_dmma_kernel: " if dmma else "nuts_euclidean_kernel: ")
+                    err = check(nuts_call(lib, m, dim, metric_kind, minv), want)
+                    if err:
+                        failures.append(f"target {target} dim {dim} metric {metric_kind} "
+                                        f"minv {minv is not None}: {err}")
+    assert not failures, f"{len(failures)} cases:\n" + "\n".join(failures[:40])
+
+
+def test_euclidean_nuts_arguments_are_checked(lib):
+    m = model(STD)
+    assert check(nuts_call(lib, m, 8, 0, None, uniforms=None), (INVALID, "null pointer")) is None
+    assert check(nuts_call(lib, m, 8, 0, None, depth=0), (INVALID, "max_tree_depth must be in")) is None
+    assert check(nuts_call(lib, m, 8, 3, None, workspace_bytes=0), (INVALID, "bad metric_kind")) is None
+    assert check(nuts_call(lib, m, 8, 0, None, workspace_bytes=0), (INVALID, "workspace too small")) is None
+    # the workspace is checked before the model's target
+    assert check(nuts_call(lib, model(UNKNOWN_TARGET), 8, 0, None, workspace_bytes=0),
+                 (INVALID, "workspace too small")) is None
+    assert check(nuts_call(lib, model(BANANA), 7, 0, None, workspace_bytes=0),
+                 (INVALID, "workspace too small")) is None
+
+
+NUTS_GENERIC_KERNELS = ("begin", "start", "leaf", "finish", "end")
+
+
+def nuts_generic_call(lib, step, n, dim, opts, ws=PTR, cs=PTR, ws_bytes=1 << 40):
+    o = ctypes.byref(opts) if opts is not None else None
+    if step == "begin":
+        return call(lib, "mb200_nuts_generic_begin", PTR, PTR, PTR, PTR, n, dim, o, ws, ws_bytes, cs,
+                    1 << 40, None)
+    if step == "start":
+        return call(lib, "mb200_nuts_generic_start", n, dim, 2, o, ws, cs, PTR, PTR, PTR, PTR, None)
+    if step == "leaf":
+        return call(lib, "mb200_nuts_generic_leaf", PTR, PTR, PTR, PTR, PTR, n, dim, 0, 4, o, ws, cs,
+                    PTR, None)
+    if step == "finish":
+        return call(lib, "mb200_nuts_generic_finish", n, dim, 2, o, ws, cs, None)
+    return call(lib, "mb200_nuts_generic_end", n, dim, o, ws, cs, *[PTR] * 10, None)
+
+
+@pytest.mark.parametrize("step", NUTS_GENERIC_KERNELS)
+def test_nuts_generic_arguments_are_checked(lib, step):
+    opts = _lib.NutsOptions(6, 0, 0, 0, 1000.0, PTR, 8)
+    bad_depth = _lib.NutsOptions(0, 0, 0, 0, 1000.0, PTR, 8)
+    no_uniforms = _lib.NutsOptions(6, 0, 0, 0, 1000.0, None, 8)
+    failures = []
+    for dim in EUCLID_DIMS:
+        cases = [
+            ((4, dim, opts), (INVALID, "bad sizes") if dim > 1024 else (CUDA, f"nuts_generic_{step}_kernel: ")),
+            ((0, dim, None), (0, None)),
+            ((4, dim, None), (INVALID, "null pointer")),
+            ((4, dim, no_uniforms), (INVALID, "null pointer")),
+            ((4, dim, bad_depth), (INVALID, "bad sizes") if dim > 1024 else (INVALID, "max_tree_depth")),
+        ]
+        for args, want in cases:
+            err = check(nuts_generic_call(lib, step, *args), want)
+            if err:
+                failures.append(f"dim {dim} {args}: {err}")
+        err = check(nuts_generic_call(lib, step, 4, dim, opts, ws=None), (INVALID, "null pointer"))
+        if err:
+            failures.append(f"dim {dim} null workspace: {err}")
+    if step == "begin":
+        err = check(nuts_generic_call(lib, step, 4, 8, opts, ws_bytes=0), (INVALID, "workspace / chain"))
+        if err:
+            failures.append(f"small workspace: {err}")
+    assert not failures, f"{len(failures)} cases:\n" + "\n".join(failures[:40])
