@@ -396,6 +396,58 @@ int mb200_project_onto_cotangent_space_gaussian(const double* pos, const double*
                                                 double* mom_out, int64_t n_chains, int32_t dim,
                                                 int32_t metric_kind, const double* metric_inv,
                                                 const mb200_model* model, void* stream);
+
+/*
+ * User-written constraints (mici_b200/csrc/user_constraint.cuh): a model's target and constraint
+ * device functions compiled at run time, by NVRTC, together with the Euclidean kernels of
+ * mb200_user_target_load and the constrained leapfrog and projection kernels.
+ *  - mb200_user_constraint_load: as mb200_user_target_load, for an image of `n_names` = 14
+ *    kernels: the 10 of mb200_user_target_load, then, with T = UserConstrainedTarget,
+ *    constrained_leapfrog_kernel<T, kp, false>, constrained_leapfrog_kernel<T, kp, true>,
+ *    constrained_project_kernel<T, kp, false>, constrained_project_kernel<T, kp, true>.
+ *    n_constr (1 .. 8) and kp (1, 2 or 4) are those the image was compiled for; mhp_constr != 0
+ *    when it defines mhp_constr.  The handle also serves the Euclidean *_user entry points and is
+ *    released by mb200_user_target_unload.
+ *  - mb200_constrained_leapfrog_euclidean_user, mb200_constrained_leapfrog_gaussian_euclidean_user,
+ *    mb200_project_onto_cotangent_space_user, mb200_project_onto_cotangent_space_gaussian_user:
+ *    the contracts of the entry points without `_user`, for model->target_id ==
+ *    MB200_TARGET_USER and a `user_target` from mb200_user_constraint_load.  dim <= 256 with one
+ *    constraint, dim <= 128 with several, and dim must select the image's kp (1: dim <= 64,
+ *    2: dim <= 128, 4: dim <= 256).  The Lebesgue density and the Gaussian system need an image
+ *    with mhp_constr.
+ */
+int mb200_user_constraint_load(const void* image, int64_t image_bytes, const char* const* names,
+                               int32_t n_names, int32_t n_constr, int32_t kp, int32_t mhp_constr,
+                               void** handle);
+int mb200_constrained_leapfrog_euclidean_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream, const void* user_target);
+int mb200_constrained_leapfrog_gaussian_euclidean_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const double* metric_omega, const double* metric_eigvec,
+    const double* metric_eigvec_t, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream, const void* user_target);
+int mb200_project_onto_cotangent_space_user(const double* pos, const double* mom_in,
+                                            double* mom_out, int64_t n_chains, int32_t dim,
+                                            int32_t metric_kind, const double* metric_inv,
+                                            const mb200_model* model, void* stream,
+                                            const void* user_target);
+int mb200_project_onto_cotangent_space_gaussian_user(const double* pos, const double* mom_in,
+                                                     double* mom_out, int64_t n_chains,
+                                                     int32_t dim, int32_t metric_kind,
+                                                     const double* metric_inv,
+                                                     const mb200_model* model, void* stream,
+                                                     const void* user_target);
+
 int mb200_sample_momentum_riemannian(const double* pos, const double* normals, double* mom_out,
                                      int64_t n_chains, int32_t dim, const mb200_model* model,
                                      int32_t* status, void* stream);

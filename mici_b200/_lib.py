@@ -106,6 +106,22 @@ SIGNATURES = {
     "mb200_project_onto_cotangent_space": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P]),
     "mb200_project_onto_cotangent_space_gaussian": (
         ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P]),
+    "mb200_user_constraint_load": (
+        ctypes.c_int, [ctypes.c_char_p, _I64, _P, _I32, _I32, _I32, _I32, _P]),
+    "mb200_constrained_leapfrog_euclidean_user": (
+        ctypes.c_int,
+        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _MP]
+        + [_I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P, _P],
+    ),
+    "mb200_constrained_leapfrog_gaussian_euclidean_user": (
+        ctypes.c_int,
+        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _P, _P, _P, _MP]
+        + [_I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P, _P],
+    ),
+    "mb200_project_onto_cotangent_space_user": (
+        ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P, _P]),
+    "mb200_project_onto_cotangent_space_gaussian_user": (
+        ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P, _P]),
     "mb200_sample_momentum_riemannian": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _MP, _P, _P]),
     "mb200_dh_dmom_riemannian": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _MP, _P, _P]),
     "mb200_selftest_dense_factor": (ctypes.c_int, [_P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),

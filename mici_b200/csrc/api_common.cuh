@@ -240,6 +240,18 @@ int eu_dispatch(const ModelArgs& m, int dim, int metric_kind, const L& l) {
   return fail(MB200_ERR_UNSUPPORTED, "target %d not available for Euclidean systems", m.target_id);
 }
 
+// The constrained kernels of a user image loaded by mb200_user_constraint_load, compiled for
+// n_constr constraints at kp, indexed by GAUSS.  n_constr == 0: an image of
+// mb200_user_target_load, which carries none.
+struct UserConstraintKernels {
+  int n_constr, kp;
+  bool mhp_constr;
+  const void* leapfrog[2];
+  const void* project[2];
+};
+// the constrained part of a loaded user image (api_euclid.cu)
+const UserConstraintKernels& user_constraint_kernels(const void* handle);
+
 // Arguments of one implicit-integrator launch on a Riemannian system (leapfrog or midpoint steps;
 // zero steps evaluate the Hamiltonian only).  ws / ws_bytes: the caller's workspace, or NULL.
 struct ImplicitArgs {

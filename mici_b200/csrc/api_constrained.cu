@@ -28,22 +28,67 @@ struct CsShape {
   static constexpr int KP = KP_;
   template <bool GAUSS>
   static size_t smem() {
-    return (size_t)CS_WARPS * constrained_smem_per_warp<T::NC, KP, GAUSS>() * sizeof(double);
+    return (size_t)CS_WARPS * cs_smem_per_warp<T, KP, GAUSS>() * sizeof(double);
   }
 };
 
-// Target / size dispatch shared by the constrained entry points: `launch(CsShape<Target, KP>{})`
-// starts the operation's kernel
+// The same for the kernels of a user image (UserConstrainedTarget): the metric product's rows and
+// the user constraint's staging area
+template <bool GAUSS>
+static size_t cs_user_smem(const UserConstraintKernels& u) {
+  return (size_t)CS_WARPS *
+         (constrained_smem_doubles(u.n_constr, u.kp, GAUSS) +
+          user_constraint_stage_per_warp(u.n_constr, u.kp)) *
+         sizeof(double);
+}
+
+// A constrained operation for constrained_target_dispatch: `registry(CsShape<Target, KP>{})`
+// starts its library kernel, `image(u)` the same kernel from the loaded user image `user` (NULL
+// for a registry target)
+template <class Registry, class Image>
+struct CsLaunch {
+  const UserConstraintKernels* user;
+  Registry registry;
+  Image image;
+};
+template <class Registry, class Image>
+static CsLaunch<Registry, Image> cs_launch(const void* user_target, Registry registry,
+                                           Image image) {
+  return {user_target ? &user_constraint_kernels(user_target) : nullptr, registry, image};
+}
+
+// Target / size dispatch shared by the constrained entry points.  A user image serves
+// dim <= 256 with one constraint and dim <= 128 with several, at the KP the sphere and
+// multi-sphere targets use for that dim, which must be the KP it was compiled for.
 template <class Launch>
 static int constrained_target_dispatch(const ModelArgs& m, int dim, const Launch& launch) {
+  if (launch.user != nullptr) {
+    const UserConstraintKernels& u = *launch.user;
+    if (m.target_id != MB200_TARGET_USER)
+      return fail(MB200_ERR_INVALID_ARG,
+                  "user-target entry point needs target_id MB200_TARGET_USER");
+    if (u.n_constr < 1)
+      return fail(MB200_ERR_INVALID_ARG,
+                  "user target has no constraint kernels (mb200_user_constraint_load)");
+    const int max_dim = u.n_constr == 1 ? 256 : 128;
+    if (dim > max_dim)
+      return fail(MB200_ERR_UNSUPPORTED, "user constraint: dim %d > %d not supported", dim,
+                  max_dim);
+    const int kp = dim <= 64 ? 1 : (dim <= 128 ? 2 : 4);
+    if (kp != u.kp)
+      return fail(MB200_ERR_INVALID_ARG, "user constraint image has kp %d; dim %d needs kp %d",
+                  u.kp, dim, kp);
+    return launch.image(u);
+  }
+  const auto& launch_registry = launch.registry;
   switch (m.target_id) {
     case MB200_TARGET_TORUS:
       if (dim != 3) return fail(MB200_ERR_INVALID_ARG, "torus target needs dim == 3");
-      return launch(CsShape<TorusTarget, 1>{});
+      return launch_registry(CsShape<TorusTarget, 1>{});
     case MB200_TARGET_SPHERE:
-      if (dim <= 64) return launch(CsShape<SphereTarget, 1>{});
-      if (dim <= 128) return launch(CsShape<SphereTarget, 2>{});
-      if (dim <= 256) return launch(CsShape<SphereTarget, 4>{});
+      if (dim <= 64) return launch_registry(CsShape<SphereTarget, 1>{});
+      if (dim <= 128) return launch_registry(CsShape<SphereTarget, 2>{});
+      if (dim <= 256) return launch_registry(CsShape<SphereTarget, 4>{});
       return fail(MB200_ERR_UNSUPPORTED, "sphere target: dim %d > 256 not supported", dim);
     case MB200_TARGET_MULTI_SPHERE: {
       const int nc = (int)m.tp[0];
@@ -51,13 +96,13 @@ static int constrained_target_dispatch(const ModelArgs& m, int dim, const Launch
         return fail(MB200_ERR_UNSUPPORTED,
                     "multi-sphere target: n_constr must be 2, 4 or 8, dim a multiple <= 128");
       if (dim <= 64) {
-        if (nc == 2) return launch(CsShape<MultiSphereTarget<2>, 1>{});
-        if (nc == 4) return launch(CsShape<MultiSphereTarget<4>, 1>{});
-        return launch(CsShape<MultiSphereTarget<8>, 1>{});
+        if (nc == 2) return launch_registry(CsShape<MultiSphereTarget<2>, 1>{});
+        if (nc == 4) return launch_registry(CsShape<MultiSphereTarget<4>, 1>{});
+        return launch_registry(CsShape<MultiSphereTarget<8>, 1>{});
       }
-      if (nc == 2) return launch(CsShape<MultiSphereTarget<2>, 2>{});
-      if (nc == 4) return launch(CsShape<MultiSphereTarget<4>, 2>{});
-      return launch(CsShape<MultiSphereTarget<8>, 2>{});
+      if (nc == 2) return launch_registry(CsShape<MultiSphereTarget<2>, 2>{});
+      if (nc == 4) return launch_registry(CsShape<MultiSphereTarget<4>, 2>{});
+      return launch_registry(CsShape<MultiSphereTarget<8>, 2>{});
     }
     default:
       return fail(MB200_ERR_UNSUPPORTED, "target %d defines no constraint", m.target_id);
@@ -74,7 +119,8 @@ static int constrained_leapfrog_dispatch(
     const double* metric_inv, const GaussianArgs& ga, const mb200_model* model,
     int32_t projection_solver, double constraint_tol, double position_tol, double divergence_tol,
     int32_t max_iters, int32_t max_line_search_iters, double reverse_check_tol, double* h_out,
-    int32_t* status, int32_t* n_done, int32_t* newton_iters, void* stream) {
+    int32_t* status, int32_t* n_done, int32_t* newton_iters, void* stream,
+    const void* user_target = nullptr) {
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
@@ -106,7 +152,7 @@ static int constrained_leapfrog_dispatch(
         n_done, newton_iters, lanes);
     return check_launch("constrained_torus_thread_kernel");
   }
-  return constrained_target_dispatch(m, dim, [&](auto shape) {
+  auto registry = [&](auto shape) {
     using S = decltype(shape);
     constrained_leapfrog_kernel<typename S::Target, S::KP, GAUSS>
         <<<cs_blocks(n_chains, CS_WARPS), CS_WARPS * 32, S::template smem<GAUSS>(), st>>>(
@@ -115,13 +161,30 @@ static int constrained_leapfrog_dispatch(
             divergence_tol, max_iters, reverse_check_tol, h_out, status, n_done, newton_iters,
             projection_solver, max_line_search_iters, ga.omega, ga.eigvec, ga.eigvec_t);
     return check_launch("constrained_leapfrog_kernel");
-  });
+  };
+  auto image = [&](const UserConstraintKernels& u) {
+    // the Lebesgue density's gradient and the Gaussian system run the matrix-Hessian product
+    if (!u.mhp_constr && (GAUSS || m.tp[MB200_MAX_PARAMS - 1] != 0.0))
+      return fail(MB200_ERR_INVALID_ARG,
+                  "user constraint defines no mhp_constr, which the %s needs",
+                  GAUSS ? "Gaussian system" : "Lebesgue density");
+    using Kernel = decltype(&constrained_leapfrog_kernel<SphereTarget, 1, GAUSS>);
+    return eu_launch(reinterpret_cast<Kernel>(u.leapfrog[GAUSS]), "constrained_leapfrog_kernel",
+                     (n_chains + CS_WARPS - 1) / CS_WARPS, 16, CS_WARPS * 32,
+                     cs_user_smem<GAUSS>(u), st, pos_in, mom_in, pos_out, mom_out, dir, n_chains,
+                     dim, step_size, n_steps, n_inner_step, metric_kind, metric_inv, m,
+                     constraint_tol, position_tol, divergence_tol, max_iters, reverse_check_tol,
+                     h_out, status, n_done, newton_iters, projection_solver,
+                     max_line_search_iters, ga.omega, ga.eigvec, ga.eigvec_t);
+  };
+  return constrained_target_dispatch(m, dim, cs_launch(user_target, registry, image));
 }
 
 template <bool GAUSS>
 static int project_dispatch(const double* pos, const double* mom_in, double* mom_out,
                             int64_t n_chains, int32_t dim, int32_t metric_kind,
-                            const double* metric_inv, const mb200_model* model, void* stream) {
+                            const double* metric_inv, const mb200_model* model, void* stream,
+                            const void* user_target = nullptr) {
   if (n_chains == 0 && dim >= 1) return 0;
   if (!pos || !mom_in || !mom_out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
@@ -130,13 +193,21 @@ static int project_dispatch(const double* pos, const double* mom_in, double* mom
     return fail(MB200_ERR_INVALID_ARG, "metric_inv is NULL");
   const DeviceScope device_scope(pos);
   const ModelArgs m = to_args(model);
-  return constrained_target_dispatch(m, dim, [&](auto shape) {
+  auto registry = [&](auto shape) {
     using S = decltype(shape);
     constrained_project_kernel<typename S::Target, S::KP, GAUSS>
         <<<cs_blocks(n_chains, CS_WARPS), CS_WARPS * 32, S::template smem<GAUSS>(),
            (cudaStream_t)stream>>>(pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv, m);
     return check_launch("constrained_project_kernel");
-  });
+  };
+  auto image = [&](const UserConstraintKernels& u) {
+    using Kernel = decltype(&constrained_project_kernel<SphereTarget, 1, GAUSS>);
+    return eu_launch(reinterpret_cast<Kernel>(u.project[GAUSS]), "constrained_project_kernel",
+                     (n_chains + CS_WARPS - 1) / CS_WARPS, 16, CS_WARPS * 32,
+                     cs_user_smem<GAUSS>(u), (cudaStream_t)stream, pos, mom_in, mom_out, n_chains,
+                     dim, metric_kind, metric_inv, m);
+  };
+  return constrained_target_dispatch(m, dim, cs_launch(user_target, registry, image));
 }
 
 }  // namespace mb200
@@ -191,6 +262,62 @@ int mb200_project_onto_cotangent_space_gaussian(const double* pos, const double*
                                                 const mb200_model* model, void* stream) {
   return project_dispatch<true>(pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv,
                                 model, stream);
+}
+
+int mb200_constrained_leapfrog_euclidean_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream, const void* user_target) {
+  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  return constrained_leapfrog_dispatch<false>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, n_inner_step, metric_kind, metric_inv, GaussianArgs{nullptr, nullptr, nullptr},
+      model, projection_solver, constraint_tol, position_tol, divergence_tol, max_iters,
+      max_line_search_iters, reverse_check_tol, h_out, status, n_done, newton_iters, stream,
+      user_target);
+}
+
+int mb200_constrained_leapfrog_gaussian_euclidean_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, int32_t n_inner_step, int32_t metric_kind,
+    const double* metric_inv, const double* metric_omega, const double* metric_eigvec,
+    const double* metric_eigvec_t, const mb200_model* model, int32_t projection_solver,
+    double constraint_tol, double position_tol, double divergence_tol, int32_t max_iters,
+    int32_t max_line_search_iters, double reverse_check_tol, double* h_out, int32_t* status,
+    int32_t* n_done, int32_t* newton_iters, void* stream, const void* user_target) {
+  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  return constrained_leapfrog_dispatch<true>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, n_inner_step, metric_kind, metric_inv,
+      GaussianArgs{metric_omega, metric_eigvec, metric_eigvec_t}, model, projection_solver,
+      constraint_tol, position_tol, divergence_tol, max_iters, max_line_search_iters,
+      reverse_check_tol, h_out, status, n_done, newton_iters, stream, user_target);
+}
+
+int mb200_project_onto_cotangent_space_user(const double* pos, const double* mom_in,
+                                            double* mom_out, int64_t n_chains, int32_t dim,
+                                            int32_t metric_kind, const double* metric_inv,
+                                            const mb200_model* model, void* stream,
+                                            const void* user_target) {
+  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  return project_dispatch<false>(pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv,
+                                 model, stream, user_target);
+}
+
+int mb200_project_onto_cotangent_space_gaussian_user(const double* pos, const double* mom_in,
+                                                     double* mom_out, int64_t n_chains,
+                                                     int32_t dim, int32_t metric_kind,
+                                                     const double* metric_inv,
+                                                     const mb200_model* model, void* stream,
+                                                     const void* user_target) {
+  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  return project_dispatch<true>(pos, mom_in, mom_out, n_chains, dim, metric_kind, metric_inv,
+                                model, stream, user_target);
 }
 
 }  // extern "C"

@@ -111,7 +111,45 @@ struct UserKernels {
   cudaLibrary_t lib;
   LeapfrogKernel leapfrog[N_EU_LAYOUTS];
   EvalKernel eval[N_EU_LAYOUTS];
+  UserConstraintKernels constr;  // mb200_user_constraint_load only
 };
+
+const UserConstraintKernels& user_constraint_kernels(const void* handle) {
+  return static_cast<const UserKernels*>(handle)->constr;
+}
+
+// Loads `image` and looks up its kernels: the Euclidean table, then (n_names > 2 N_EU_LAYOUTS)
+// the constrained one, in the order of include/mici_b200.h
+static int user_image_load(const void* image, const char* const* names, int n_names,
+                           const UserConstraintKernels& constr, void** handle) {
+  UserKernels* u = new UserKernels();
+  u->constr = constr;
+  cudaError_t e = cudaLibraryLoadData(&u->lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0);
+  if (e != cudaSuccess) {
+    delete u;
+    return fail(MB200_ERR_CUDA, "cudaLibraryLoadData: %s", cudaGetErrorString(e));
+  }
+  for (int i = 0; i < n_names; ++i) {
+    cudaKernel_t k;
+    e = cudaLibraryGetKernel(&k, u->lib, names[i]);
+    if (e != cudaSuccess) {
+      cudaLibraryUnload(u->lib);
+      delete u;
+      return fail(MB200_ERR_CUDA, "cudaLibraryGetKernel(%s): %s", names[i], cudaGetErrorString(e));
+    }
+    const int c = i - 2 * N_EU_LAYOUTS;
+    if (i < N_EU_LAYOUTS)
+      u->leapfrog[i] = reinterpret_cast<LeapfrogKernel>(k);
+    else if (c < 0)
+      u->eval[i - N_EU_LAYOUTS] = reinterpret_cast<EvalKernel>(k);
+    else if (c < 2)
+      u->constr.leapfrog[c] = reinterpret_cast<const void*>(k);
+    else
+      u->constr.project[c - 2] = reinterpret_cast<const void*>(k);
+  }
+  *handle = u;
+  return 0;
+}
 
 // Splitting schedule of the C-ABI arguments: n_flows (odd) coefficients alternating a, b, ..., a
 // with a = h1_flow (kick) if initial_h1_flow_step else h2_flow (drift) (integrators.py:268-281);
@@ -333,27 +371,21 @@ int mb200_user_target_load(const void* image, int64_t image_bytes, const char* c
   if (n_names != 2 * N_EU_LAYOUTS)
     return fail(MB200_ERR_INVALID_ARG, "expected %d kernel names, got %d", 2 * N_EU_LAYOUTS,
                 n_names);
-  UserKernels* u = new UserKernels();
-  cudaError_t e = cudaLibraryLoadData(&u->lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0);
-  if (e != cudaSuccess) {
-    delete u;
-    return fail(MB200_ERR_CUDA, "cudaLibraryLoadData: %s", cudaGetErrorString(e));
-  }
-  for (int i = 0; i < n_names; ++i) {
-    cudaKernel_t k;
-    e = cudaLibraryGetKernel(&k, u->lib, names[i]);
-    if (e != cudaSuccess) {
-      cudaLibraryUnload(u->lib);
-      delete u;
-      return fail(MB200_ERR_CUDA, "cudaLibraryGetKernel(%s): %s", names[i], cudaGetErrorString(e));
-    }
-    if (i < N_EU_LAYOUTS)
-      u->leapfrog[i] = reinterpret_cast<LeapfrogKernel>(k);
-    else
-      u->eval[i - N_EU_LAYOUTS] = reinterpret_cast<EvalKernel>(k);
-  }
-  *handle = u;
-  return 0;
+  return user_image_load(image, names, n_names, UserConstraintKernels{}, handle);
+}
+
+int mb200_user_constraint_load(const void* image, int64_t image_bytes, const char* const* names,
+                               int32_t n_names, int32_t n_constr, int32_t kp, int32_t mhp_constr,
+                               void** handle) {
+  if (!image || image_bytes <= 0 || !names || !handle)
+    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_names != 2 * N_EU_LAYOUTS + 4)
+    return fail(MB200_ERR_INVALID_ARG, "expected %d kernel names, got %d", 2 * N_EU_LAYOUTS + 4,
+                n_names);
+  if (n_constr < 1 || n_constr > 8 || (kp != 1 && kp != 2 && kp != 4))
+    return fail(MB200_ERR_INVALID_ARG, "n_constr must be in [1, 8] and kp 1, 2 or 4");
+  return user_image_load(image, names, n_names,
+                         UserConstraintKernels{n_constr, kp, mhp_constr != 0, {}, {}}, handle);
 }
 
 int mb200_user_target_unload(void* handle) {

@@ -24,6 +24,9 @@ namespace mb200 {
 //   grad(lane, dim, q, g)               gradient of l
 //   nld(lane, dim, q)                   l(q), same value on all lanes
 //   constr_jacob(lane, dim, q, c, J)    c(q) [NC] on all lanes; J[NC][NV] columns owned by lane
+//   mhp(lane, dim, q, m, out)           out_j = sum_{k,i} m[k][i] d^2 c_k / dq_i dq_j
+// User-written constraints implement the same interface (UserConstrainedTarget,
+// user_constraint.cuh).
 // ---------------------------------------------------------------------------------------------
 
 // Torus in R^3 (reference README.md:315-337): rho = sqrt(x^2+y^2), theta = atan2(y, x),
@@ -874,9 +877,41 @@ struct ConstrainedOps {
 
 // Shared-memory doubles per warp: the rows staged by the dense metric product (C of them; the
 // Gaussian split also rotates q and p together)
+__host__ __device__ constexpr int constrained_smem_doubles(int c, int kp, bool gauss) {
+  return (c > 1 ? c : (gauss ? 2 : 1)) * 64 * kp;
+}
 template <int C, int KP, bool GAUSS>
 __host__ __device__ constexpr int constrained_smem_per_warp() {
-  return (C > 1 ? C : (GAUSS ? 2 : 1)) * 64 * KP;
+  return constrained_smem_doubles(C, KP, GAUSS);
+}
+
+// A user-written constraint (user_constraint.cuh) declares STAGED = true: it sees whole vectors
+// and stages each chain's q, NC rows of J (or of the matrix-Hessian product's operand) and one
+// output vector through per-warp shared memory of its own, after the metric product's.  Registry
+// targets declare nothing and get nothing.
+template <class T>
+__host__ __device__ constexpr auto cs_staged(int) -> decltype(T::STAGED) {
+  return T::STAGED;
+}
+template <class T>
+__host__ __device__ constexpr bool cs_staged(long) {
+  return false;
+}
+__host__ __device__ constexpr int user_constraint_stage_per_warp(int nc, int kp) {
+  return (nc + 2) * 64 * kp;
+}
+template <class Target, int KP, bool GAUSS>
+__host__ __device__ constexpr int cs_smem_per_warp() {
+  return constrained_smem_per_warp<Target::NC, KP, GAUSS>() +
+         (cs_staged<Target>(0) ? user_constraint_stage_per_warp(Target::NC, KP) : 0);
+}
+// The kernel's target; a staged one gets its area, behind the metric product's in `warp_smem`
+template <class Target, int KP, bool GAUSS>
+__device__ __forceinline__ Target cs_target(const ModelArgs& m, int dim, double* warp_smem) {
+  if constexpr (cs_staged<Target>(0))
+    return Target(m, dim, warp_smem + constrained_smem_per_warp<Target::NC, KP, GAUSS>());
+  else
+    return Target(m, dim);
 }
 
 // GAUSS selects the flow policy of GaussianDenseConstrainedEuclideanMetricSystem
@@ -898,12 +933,13 @@ __global__ void __launch_bounds__(128)
                                 const double* __restrict__ eigvec,
                                 const double* __restrict__ eigvec_t) {
   constexpr int NV = 2 * KP;
-  constexpr int SM_PER_WARP = constrained_smem_per_warp<Target::NC, KP, GAUSS>();
+  constexpr int SM_PER_WARP = cs_smem_per_warp<Target, KP, GAUSS>();
   extern __shared__ double smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int wpb = blockDim.x >> 5;
-  const Target target(model, dim);
+  const Target target =
+      cs_target<Target, KP, GAUSS>(model, dim, smem + (size_t)warp * SM_PER_WARP);
   ConstrainedOps<Target, KP, GAUSS> ops{target,      metric_kind,
                                         minv,        dim,
                                         lane,        smem + (size_t)warp * SM_PER_WARP,
@@ -1048,12 +1084,13 @@ __global__ void __launch_bounds__(128)
                                int64_t n_chains, int dim, int metric_kind,
                                const double* __restrict__ minv, ModelArgs model) {
   constexpr int NV = 2 * KP;
-  constexpr int SM_PER_WARP = constrained_smem_per_warp<Target::NC, KP, GAUSS>();
+  constexpr int SM_PER_WARP = cs_smem_per_warp<Target, KP, GAUSS>();
   extern __shared__ double smem[];
   const int lane = threadIdx.x & 31;
   const int warp = threadIdx.x >> 5;
   const int wpb = blockDim.x >> 5;
-  const Target target(model, dim);
+  const Target target =
+      cs_target<Target, KP, GAUSS>(model, dim, smem + (size_t)warp * SM_PER_WARP);
   const ConstrainedOps<Target, KP, GAUSS> ops{target, metric_kind, minv, dim, lane,
                                               smem + (size_t)warp * SM_PER_WARP, 0, 0};
   for (int64_t ch = (int64_t)blockIdx.x * wpb + warp; ch < n_chains;

@@ -52,6 +52,7 @@ from .systems import (
     _batched,
     _dir_tensor,
     _like_input,
+    _user_entry,
 )
 
 
@@ -566,6 +567,7 @@ class ConstrainedLeapfrogIntegrator(TractableFlowIntegrator):
             metric += tuple(_lib.ptr(a) for a in sysm.rotation_args(dev))
         else:
             entry = "mb200_constrained_leapfrog_euclidean"
+        entry, user = _user_entry(entry, sysm.target)
         rc = getattr(_lib.load(), entry)(
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
             n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), int(self.n_inner_step),
@@ -574,6 +576,7 @@ class ConstrainedLeapfrogIntegrator(TractableFlowIntegrator):
             float(kw["divergence_tol"]), int(kw["max_iters"]),
             int(kw.get("max_line_search_iters", 10)), float(self.reverse_check_tol), _lib.ptr(h),
             _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters), _lib.current_stream_ptr(dev),
+            *user,
         )
         _lib.check(rc, entry)
         return iters

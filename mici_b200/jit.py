@@ -9,6 +9,11 @@ works anywhere.  The library itself never links NVRTC.
 Compiled images and loaded handles live in one process-wide cache keyed by a hash of the
 headers, the user source, the options and the NVRTC version (nothing is written to disk), so
 that system and integrator objects hold only the source and survive ``deepcopy`` / pickling.
+
+A constrained user target (``n_constr >= 1``, contract: ``csrc/user_constraint.cuh``) also
+carries the constrained leapfrog and projection kernels (``csrc/constrained.cuh``) for its
+constraint count and KP; its cache key covers both and whether the source defines
+``mhp_constr``.
 """
 
 from __future__ import annotations
@@ -37,12 +42,31 @@ NAME_EXPRESSIONS = tuple(
     + [f"&mb200::euclidean_eval_kernel<mb200::UserTarget, {kp}>" for kp, _ in LAYOUTS]
 )
 
+
+def constrained_name_expressions(kp):
+    """The kernels a constrained image carries after NAME_EXPRESSIONS, in the kernel-table order
+    of ``mb200_user_constraint_load``: leapfrog then projection, each with GAUSS false then true
+    (GaussianDenseConstrainedEuclideanMetricSystem)."""
+    t = "mb200::UserConstrainedTarget"
+    return tuple(f"&mb200::constrained_{k}_kernel<{t}, {kp}, {g}>"
+                 for k in ("leapfrog", "project") for g in ("false", "true"))
+
+
+def constrained_kp(dim, n_constr):
+    """KP (coordinates per lane / 2) of the constrained kernel for ``dim``, chosen as for the
+    registry's sphere and multi-sphere targets; ``None`` outside dim <= 256 (one constraint) or
+    dim <= 128 (several)."""
+    if dim > (256 if n_constr == 1 else 128):
+        return None
+    return 1 if dim <= 64 else (2 if dim <= 128 else 4)
+
 _lock = threading.Lock()
 _nvrtc = None
 _images = {}   # key -> (cubin bytes, lowered names)
 _handles = {}  # key -> loaded library handle (ctypes.c_void_p)
-# (source, name) -> key / handle: a repeat lookup, once per launch of a user target, is one dict
-# access; the headers are hashed and NVRTC's version read once per process (_static_key)
+# (source, name, constraint) -> key / handle: a repeat lookup, once per launch of a user target,
+# is one dict access; the headers are hashed and NVRTC's version read once per process
+# (_static_key).  constraint: () for an unconstrained target, else (n_constr, kp, mhp_constr).
 _keys = {}
 _loaded = {}
 _static = None
@@ -134,10 +158,30 @@ def _headers_digest():
     return h.hexdigest()
 
 
-def translation_unit(source, name="user_target"):
+def translation_unit(source, name="user_target", constraint=()):
     """The program NVRTC compiles: the engine header, then the user source with its own line
     numbers (``#line``), so that compile errors point at the user's lines."""
-    return f'#include "user_target.cuh"\n#line 1 "{name}.cu"\n{source}\n'
+    header = "user_constraint.cuh" if constraint else "user_target.cuh"
+    return f'#include "{header}"\n#line 1 "{name}.cu"\n{source}\n'
+
+
+def _constraint(n_constr, kp, mhp_constr):
+    if not n_constr:
+        return ()
+    if not 1 <= n_constr <= 8 or kp not in (1, 2, 4):
+        raise ValueError(f"bad constrained image: n_constr={n_constr}, kp={kp}")
+    return (int(n_constr), int(kp), bool(mhp_constr))
+
+
+def _defines(constraint):
+    if not constraint:
+        return ()
+    n_constr, _, mhp = constraint
+    return (f"-DMB200_USER_N_CONSTR={n_constr}",) + (("-DMB200_USER_MHP_CONSTR",) if mhp else ())
+
+
+def _name_expressions(constraint):
+    return NAME_EXPRESSIONS + (constrained_name_expressions(constraint[1]) if constraint else ())
 
 
 def _static_key():
@@ -149,43 +193,50 @@ def _static_key():
     return _static
 
 
-def cache_key(source, name="user_target"):
-    return hashlib.sha256("\0".join([_static_key(), name, source]).encode()).hexdigest()
+def cache_key(source, name="user_target", constraint=()):
+    parts = [_static_key(), name, source]
+    if constraint:
+        parts.append("n_constr=%d kp=%d mhp_constr=%d" % constraint)
+    return hashlib.sha256("\0".join(parts).encode()).hexdigest()
 
 
-def compile_target(source, name="user_target"):
+def compile_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=False):
     """Compile a user target; returns ``(key, cubin, lowered kernel names)``, from the process
-    cache when the same source was compiled before.  Raises ``TargetCompileError`` with the
-    NVRTC log on failure."""
+    cache when the same source was compiled before.  ``n_constr >= 1``: a constrained target,
+    whose image also carries the constrained kernels at ``kp``.  Raises ``TargetCompileError``
+    with the NVRTC log on failure."""
+    constraint = _constraint(n_constr, kp, mhp_constr)
     with _lock:
-        key = _keys.get((source, name))
+        key = _keys.get((source, name, constraint))
         if key is not None:
             stats["hits"] += 1
             return key, *_images[key]
-    key = cache_key(source, name)
+    key = cache_key(source, name, constraint)
     with _lock:
         if key in _images:  # the same program under another (source, name) spelling
             stats["hits"] += 1
-            _keys[(source, name)] = key
+            _keys[(source, name, constraint)] = key
             return key, *_images[key]
-    cubin, names = _compile(source, name)
+    cubin, names = _compile(source, name, constraint)
     with _lock:
         _images.setdefault(key, (cubin, names))
-        _keys[(source, name)] = key
+        _keys[(source, name, constraint)] = key
         stats["compiles"] += 1
         return key, *_images[key]
 
 
-def _compile(source, name):
+def _compile(source, name, constraint=()):
     lib = nvrtc()
     prog = ctypes.c_void_p()
-    src = translation_unit(source, name).encode()
+    src = translation_unit(source, name, constraint).encode()
+    exprs = _name_expressions(constraint)
     _ok(lib.nvrtcCreateProgram(ctypes.byref(prog), src, f"{name}_tu.cu".encode(), 0, None, None),
         "nvrtcCreateProgram")
     try:
-        for expr in NAME_EXPRESSIONS:
+        for expr in exprs:
             _ok(lib.nvrtcAddNameExpression(prog, expr.encode()), "nvrtcAddNameExpression")
-        opts = [o.encode() for o in OPTIONS] + [f"-I{CSRC}".encode(), f"-I{INCLUDE}".encode()]
+        opts = [o.encode() for o in OPTIONS + _defines(constraint)] + [
+            f"-I{CSRC}".encode(), f"-I{INCLUDE}".encode()]
         argv = (ctypes.c_char_p * len(opts))(*opts)
         rc = lib.nvrtcCompileProgram(prog, len(opts), ctypes.cast(argv, ctypes.c_void_p))
         log_size = ctypes.c_size_t()
@@ -202,7 +253,7 @@ def _compile(source, name):
         cubin = ctypes.create_string_buffer(size.value)
         _ok(lib.nvrtcGetCUBIN(prog, cubin), "nvrtcGetCUBIN")
         names = []
-        for expr in NAME_EXPRESSIONS:
+        for expr in exprs:
             lowered = ctypes.c_char_p()
             _ok(lib.nvrtcGetLoweredName(prog, expr.encode(), ctypes.byref(lowered)),
                 "nvrtcGetLoweredName")
@@ -212,24 +263,33 @@ def _compile(source, name):
         lib.nvrtcDestroyProgram(ctypes.byref(prog))
 
 
-def load_target(source, name="user_target"):
-    """Handle of the loaded image of a user target (``mb200_user_target_load``), compiled and
-    loaded once per process."""
+def load_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=False):
+    """Handle of the loaded image of a user target (``mb200_user_target_load``, or
+    ``mb200_user_constraint_load`` for a constrained one), compiled and loaded once per
+    process."""
     from . import _lib  # noqa: PLC0415
 
+    constraint = _constraint(n_constr, kp, mhp_constr)
     with _lock:
-        handle = _loaded.get((source, name))
+        handle = _loaded.get((source, name, constraint))
     if handle is not None:
         return handle
-    key, cubin, names = compile_target(source, name)
+    key, cubin, names = compile_target(source, name, n_constr=n_constr, kp=kp,
+                                       mhp_constr=mhp_constr)
     with _lock:
         handle = _handles.get(key)
         if handle is None:
             lib = _lib.load()
             arr = (ctypes.c_char_p * len(names))(*[n.encode() for n in names])
             handle = ctypes.c_void_p()
-            _lib.check(lib.mb200_user_target_load(cubin, len(cubin), arr, len(names),
-                                                  ctypes.byref(handle)), "mb200_user_target_load")
+            if constraint:
+                rc = lib.mb200_user_constraint_load(cubin, len(cubin), arr, len(names), *constraint,
+                                                    ctypes.byref(handle))
+                _lib.check(rc, "mb200_user_constraint_load")
+            else:
+                rc = lib.mb200_user_target_load(cubin, len(cubin), arr, len(names),
+                                                ctypes.byref(handle))
+                _lib.check(rc, "mb200_user_target_load")
             _handles[key] = handle
-        _loaded[(source, name)] = handle
+        _loaded[(source, name, constraint)] = handle
     return handle

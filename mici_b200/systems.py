@@ -440,6 +440,13 @@ class GaussianEuclideanMetricSystem(EuclideanMetricSystem):
         _gaussian_flow(self, state, dt)
 
 
+def _user_entry(entry, target):
+    """``(entry point, trailing arguments)`` of a constrained operation: the ``_user`` twin with
+    the loaded image for a ``CudaTarget``, else the registry entry point with none."""
+    user = user_handle(target)
+    return (entry, ()) if user is None else (entry + "_user", (user,))
+
+
 def _col(dt):
     return dt[..., None] if isinstance(dt, torch.Tensor) and dt.ndim >= 1 else dt
 
@@ -461,12 +468,25 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
     with respect to the Lebesgue measure and ``h1`` / ``dh1_dpos`` carry ``log det gram / 2`` and
     its gradient through the constraint's matrix-Hessian product (systems.py:853-861, 1024-1031),
     fused into the kernels.
+
+    A ``CudaTarget`` with ``n_constr >= 1`` brings its own constraint (user-written CUDA,
+    ``csrc/user_constraint.cuh``); with ``dens_wrt_hausdorff=False`` it must define
+    ``mhp_constr``.
     """
 
-    _user_targets = False
+    _user_targets = True
 
     def __init__(self, neg_log_dens, constr=None, *, metric=None, dens_wrt_hausdorff=True,
                  grad_neg_log_dens=None, jacob_constr=None, backend=None):
+        if isinstance(neg_log_dens, CudaTarget):
+            if neg_log_dens.n_constr < 1:  # the TypeError of System for an unconstrained one
+                raise TypeError(f"{type(self).__name__} does not take a CudaTarget: user targets "
+                                "run on EuclideanMetricSystem.")
+            if not dens_wrt_hausdorff and not neg_log_dens.mhp_constr:
+                raise ValueError(f"{type(self).__name__} with a density with respect to the "
+                                 "Lebesgue measure needs the constraint's matrix-Hessian "
+                                 "product: define mhp_constr and pass mhp_constr=True to "
+                                 "CudaTarget.")
         EuclideanMetricSystem.__init__(self, neg_log_dens, metric=metric,
                                        grad_neg_log_dens=grad_neg_log_dens, backend=backend)
         if constr is not None and constr is not neg_log_dens:
@@ -488,13 +508,14 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
         scratch_q, scratch_p = torch.empty_like(pos), torch.empty_like(mom)
         m = self._metric
         model = self._model(dev)
-        rc = _lib.load().mb200_constrained_leapfrog_euclidean(
+        entry, user = _user_entry("mb200_constrained_leapfrog_euclidean", self.target)
+        rc = getattr(_lib.load(), entry)(
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(scratch_q), _lib.ptr(scratch_p), None, n, dim,
             0.0, None, 0, None, 1, m.kind, _lib.ptr(m.inv_device(dev)), ctypes.byref(model), 0,
             1e-9, 1e-8, 1e10, 50, 10, 2e-8, _lib.ptr(h), None, None, None,
-            _lib.current_stream_ptr(dev),
+            _lib.current_stream_ptr(dev), *user,
         )
-        _lib.check(rc, "mb200_constrained_leapfrog_euclidean")
+        _lib.check(rc, entry)
         return _like_input(state.pos, h[0] if single else h)
 
     def project_onto_cotangent_space(self, mom, state):
@@ -518,9 +539,10 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
         m = self._metric
         minv = None if m.kind == METRIC_IDENTITY else m.inv_device(dev)
         model = self._model(dev)
+        entry, user = _user_entry(entry, self.target)
         rc = getattr(_lib.load(), entry)(
             _lib.ptr(pos_t), _lib.ptr(mom_t), _lib.ptr(out), n, dim, m.kind, _lib.ptr(minv),
-            ctypes.byref(model), _lib.current_stream_ptr(dev),
+            ctypes.byref(model), _lib.current_stream_ptr(dev), *user,
         )
         _lib.check(rc, entry)
         return _like_input(ref, out[0] if single else out)
@@ -546,7 +568,10 @@ class GaussianDenseConstrainedEuclideanMetricSystem(GaussianEuclideanMetricSyste
     conditioned on ``constr(q) == 0`` (always ``dens_wrt_hausdorff=False``).  ``h1 = l(q) +
     log det gram / 2``, ``h2 = q.q/2 + p.M^-1 p/2`` whose flow is the exact rotation in the
     eigenbasis of ``M``; the Gram matrices are inverted through their eigendecomposition.  The
-    constrained leapfrog drives it through ``mb200_constrained_leapfrog_gaussian_euclidean``."""
+    constrained leapfrog drives it through ``mb200_constrained_leapfrog_gaussian_euclidean``.
+    A constrained ``CudaTarget`` must define ``mhp_constr``."""
+
+    _user_targets = True  # GaussianEuclideanMetricSystem's False comes first in the MRO
 
     def __init__(self, neg_log_dens, constr=None, *, metric=None, grad_neg_log_dens=None,
                  jacob_constr=None, mhp_constr=None, backend=None):
@@ -586,13 +611,14 @@ class GaussianDenseConstrainedEuclideanMetricSystem(GaussianEuclideanMetricSyste
         scratch_q, scratch_p = torch.empty_like(pos), torch.empty_like(mom)
         m = self._metric
         om, u, ut = self.rotation_args(dev)
-        rc = _lib.load().mb200_constrained_leapfrog_gaussian_euclidean(
+        entry, user = _user_entry("mb200_constrained_leapfrog_gaussian_euclidean", self.target)
+        rc = getattr(_lib.load(), entry)(
             _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(scratch_q), _lib.ptr(scratch_p), None, n, dim,
             0.0, None, 0, None, 1, m.kind, _lib.ptr(m.inv_device(dev)), _lib.ptr(om), _lib.ptr(u),
             _lib.ptr(ut), ctypes.byref(self._model(dev)), 0, 1e-9, 1e-8, 1e10, 50, 10, 2e-8,
-            _lib.ptr(h), None, None, None, _lib.current_stream_ptr(dev),
+            _lib.ptr(h), None, None, None, _lib.current_stream_ptr(dev), *user,
         )
-        _lib.check(rc, "mb200_constrained_leapfrog_gaussian_euclidean")
+        _lib.check(rc, entry)
         return _like_input(state.pos, h[0] if single else h)
 
     def h2(self, state):

@@ -155,11 +155,20 @@ class CudaTarget(Target):
 
     The source compiles on first use (``compile()`` compiles now).  The instance holds only
     source, params and aux; the compiled image lives in a process-wide cache, so systems and
-    integrators holding a ``CudaTarget`` survive ``deepcopy`` and pickling."""
+    integrators holding a ``CudaTarget`` survive ``deepcopy`` and pickling.
+
+    ``n_constr >= 1`` makes it a constrained target: the source also defines ``constr`` and
+    ``jacob_constr`` over ``mb200::N_CONSTR = n_constr`` constraints, and ``mhp_constr`` when
+    ``mhp_constr=True`` (contract: ``mici_b200/csrc/user_constraint.cuh``).  It then runs on the
+    constrained Euclidean systems with ``ConstrainedLeapfrogIntegrator``: ``n_constr <= 8``,
+    ``dim <= 256`` with one constraint and ``dim <= 128`` with several, at most 7 params (the
+    last slot carries the density's measure).  The Lebesgue density (``dens_wrt_hausdorff=False``)
+    and ``GaussianDenseConstrainedEuclideanMetricSystem`` need ``mhp_constr``."""
 
     target_id = TARGET_USER
 
-    def __init__(self, dim, source, params=(), aux=None, name=None):
+    def __init__(self, dim, source, params=(), aux=None, name=None, *, n_constr=0,
+                 mhp_constr=False):
         if not isinstance(source, str):
             raise ValueError("`source` must be a string of CUDA C++.")
         dim = int(dim)
@@ -171,6 +180,18 @@ class CudaTarget(Target):
             raise ValueError(f"`params` must be an iterable of scalars: {e}") from e
         if len(params) > 8:
             raise ValueError(f"CudaTarget takes at most 8 params, got {len(params)}.")
+        if (isinstance(n_constr, bool) or not isinstance(n_constr, (int, np.integer))
+                or not 0 <= n_constr <= 8):
+            raise ValueError(f"`n_constr` must be an integer in [0, 8], got {n_constr!r}.")
+        n_constr = int(n_constr)
+        if n_constr:
+            max_dim = 256 if n_constr == 1 else 128
+            if dim > max_dim:
+                raise ValueError(f"A CudaTarget with {n_constr} constraint(s) needs dim <= "
+                                 f"{max_dim}, got {dim}.")
+            if len(params) > 7:
+                raise ValueError("A constrained CudaTarget takes at most 7 params (the last slot "
+                                 f"carries the density's measure), got {len(params)}.")
         if aux is not None:
             try:
                 aux = np.ascontiguousarray(aux, dtype=np.float64)
@@ -181,23 +202,36 @@ class CudaTarget(Target):
         self.name = "user_target" if name is None else str(name)
         if not self.name.isidentifier():
             raise ValueError("`name` must be a valid identifier.")
+        self.n_constr = n_constr
+        self.mhp_constr = bool(mhp_constr) and n_constr > 0
+
+    def _image_kwargs(self):
+        """What the image depends on besides the source: constraint count, KP, mhp_constr."""
+        if not self.n_constr:
+            return {}
+        from . import jit  # noqa: PLC0415
+
+        return {"n_constr": self.n_constr, "kp": jit.constrained_kp(self.dim, self.n_constr),
+                "mhp_constr": self.mhp_constr}
 
     def compile(self):
         """Compile now (raises ``mici_b200.errors.TargetCompileError``); returns ``self``."""
         from . import jit  # noqa: PLC0415
 
-        jit.compile_target(self.source, self.name)
+        jit.compile_target(self.source, self.name, **self._image_kwargs())
         return self
 
     def handle(self):
-        """The loaded device image (``mb200_user_target_load``) of this source, from the process
+        """The loaded device image (``mb200_user_target_load``, or
+        ``mb200_user_constraint_load`` when constrained) of this source, from the process
         cache."""
         from . import jit  # noqa: PLC0415
 
-        return jit.load_target(self.source, self.name)
+        return jit.load_target(self.source, self.name, **self._image_kwargs())
 
     def __repr__(self):
-        return f"CudaTarget(dim={self.dim}, name={self.name!r}, params={self.params})"
+        extra = f", n_constr={self.n_constr}" if self.n_constr else ""
+        return f"CudaTarget(dim={self.dim}, name={self.name!r}, params={self.params}{extra})"
 
 
 def user_handle(target):
