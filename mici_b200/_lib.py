@@ -61,6 +61,11 @@ _NP = ctypes.POINTER(NutsOptions)
 # mb200_leapfrog_euclidean and its general-kernel twin
 _LEAPFROG_EUCLIDEAN_ARGS = [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _P, _I32, _I32,
                             _P, _MP, _P, _P, _P, _P]
+# mb200_constrained_leapfrog[_gaussian]_euclidean: the Gaussian system's three rotation operands
+# follow metric_inv
+_CONSTRAINED_HEAD = [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P]
+_CONSTRAINED_TAIL = [_MP, _I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P]
+_PROJECT_ARGS = [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P]
 
 # symbol -> (restype, argtypes): every symbol declared in include/mici_b200.h
 SIGNATURES = {
@@ -73,20 +78,9 @@ SIGNATURES = {
     "mb200_euclidean_eval": (ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P, _P, _P, _P]),
     "mb200_user_target_load": (ctypes.c_int, [ctypes.c_char_p, _I64, _P, _I32, _P]),
     "mb200_user_target_unload": (ctypes.c_int, [_P]),
-    "mb200_leapfrog_euclidean_user": (ctypes.c_int, _LEAPFROG_EUCLIDEAN_ARGS + [_P]),
-    "mb200_hamiltonian_euclidean_user": (ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P, _P]),
-    "mb200_euclidean_eval_user": (
-        ctypes.c_int, [_P, _P, _I64, _I32, _I32, _P, _MP, _P, _P, _P, _P, _P, _P]),
-    "mb200_constrained_leapfrog_euclidean": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _MP]
-        + [_I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P],
-    ),
+    "mb200_constrained_leapfrog_euclidean": (ctypes.c_int, _CONSTRAINED_HEAD + _CONSTRAINED_TAIL),
     "mb200_constrained_leapfrog_gaussian_euclidean": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _P, _P, _P, _MP]
-        + [_I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P],
-    ),
+        ctypes.c_int, _CONSTRAINED_HEAD + [_P, _P, _P] + _CONSTRAINED_TAIL),
     "mb200_implicit_leapfrog_riemannian": (
         ctypes.c_int,
         [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _MP, _I32, _F64, _F64, _I32, _F64]
@@ -103,25 +97,10 @@ SIGNATURES = {
         [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _MP, _I32, _F64, _F64, _I32, _F64]
         + [_P, _P, _P, _P, _P],
     ),
-    "mb200_project_onto_cotangent_space": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P]),
-    "mb200_project_onto_cotangent_space_gaussian": (
-        ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P]),
+    "mb200_project_onto_cotangent_space": (ctypes.c_int, _PROJECT_ARGS),
+    "mb200_project_onto_cotangent_space_gaussian": (ctypes.c_int, _PROJECT_ARGS),
     "mb200_user_constraint_load": (
         ctypes.c_int, [ctypes.c_char_p, _I64, _P, _I32, _I32, _I32, _I32, _P]),
-    "mb200_constrained_leapfrog_euclidean_user": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _MP]
-        + [_I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P, _P],
-    ),
-    "mb200_constrained_leapfrog_gaussian_euclidean_user": (
-        ctypes.c_int,
-        [_P, _P, _P, _P, _P, _I64, _I32, _F64, _P, _I32, _P, _I32, _I32, _P, _P, _P, _P, _MP]
-        + [_I32, _F64, _F64, _F64, _I32, _I32, _F64, _P, _P, _P, _P, _P, _P],
-    ),
-    "mb200_project_onto_cotangent_space_user": (
-        ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P, _P]),
-    "mb200_project_onto_cotangent_space_gaussian_user": (
-        ctypes.c_int, [_P, _P, _P, _I64, _I32, _I32, _P, _MP, _P, _P]),
     "mb200_sample_momentum_riemannian": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _MP, _P, _P]),
     "mb200_dh_dmom_riemannian": (ctypes.c_int, [_P, _P, _P, _I64, _I32, _MP, _P, _P]),
     "mb200_selftest_dense_factor": (ctypes.c_int, [_P, _P, _I64, _I32, _P, _P, _P, _P, _P, _P]),
@@ -160,6 +139,13 @@ SIGNATURES = {
     "mb200_hamiltonian_riemannian": (ctypes.c_int, [_P, _P, _I64, _I32, _MP, _P, _P, _P, _I64, _P]),
 }
 
+# each `_user` twin takes its registry entry point's arguments plus the loaded image's handle
+for _name in ("mb200_leapfrog_euclidean", "mb200_hamiltonian_euclidean", "mb200_euclidean_eval",
+              "mb200_constrained_leapfrog_euclidean",
+              "mb200_constrained_leapfrog_gaussian_euclidean",
+              "mb200_project_onto_cotangent_space", "mb200_project_onto_cotangent_space_gaussian"):
+    SIGNATURES[_name + "_user"] = (SIGNATURES[_name][0], SIGNATURES[_name][1] + [_P])
+
 _lock = threading.Lock()
 _lib = None
 
@@ -187,6 +173,17 @@ def load():
                 fn.argtypes = args
             _lib = lib
     return _lib
+
+
+def call(entry, *args, target=None):
+    """Call the entry point ``entry`` and raise if it fails.  For a user-written ``CudaTarget``
+    it calls the ``_user`` twin instead, with the target's loaded image appended."""
+    from .targets import user_handle  # noqa: PLC0415
+
+    user = user_handle(target)
+    if user is not None:
+        entry, args = entry + "_user", (*args, user)
+    check(getattr(load(), entry)(*args), entry)
 
 
 def check(rc: int, what: str) -> None:

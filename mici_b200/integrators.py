@@ -42,17 +42,16 @@ _FUSED_PROJECTION_SOLVERS = (
     solve_projection_onto_manifold_newton_with_line_search,
 )
 from .states import ChainState
-from .targets import CudaTarget, user_handle
 from .systems import (
     ConstrainedEuclideanMetricSystem,
     EuclideanMetricSystem,
-    GaussianDenseConstrainedEuclideanMetricSystem,
     GaussianEuclideanMetricSystem,
     RiemannianMetricSystem,
     _batched,
     _dir_tensor,
     _like_input,
-    _user_entry,
+    _on_batch,
+    _registry_euclidean,
 )
 
 
@@ -104,8 +103,6 @@ class Integrator(ABC):
         pos, mom, d, single = _batched(state)
         n, dim = pos.shape
         dev = pos.device
-        pos = pos.contiguous()
-        mom = mom.contiguous()
         pos_out = torch.empty_like(pos)
         mom_out = torch.empty_like(mom)
         status = torch.empty(n, dtype=torch.int32, device=dev)
@@ -258,19 +255,13 @@ class TractableFlowIntegrator(Integrator):
         eps, eps_t, ns, max_n = _step_args(self.step_size, n_steps, n, dev)
         coefs, n_flows = _coefficients_arg(self.coefficients)
         model = sysm._model(dev)
-        args = (
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), n_flows, coefs,
-            1 if self.initial_h1_flow_step else 0, sysm.metric.kind,
+        # a user-written target runs the general-dimension kernel of its run-time compiled image
+        _lib.call(
+            "mb200_leapfrog_euclidean", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out),
+            _lib.ptr(mom_out), _lib.ptr(dirs), n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns),
+            n_flows, coefs, 1 if self.initial_h1_flow_step else 0, sysm.metric.kind,
             _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model), _lib.ptr(h),
-            _lib.ptr(status), _lib.ptr(n_done), _lib.current_stream_ptr(dev),
-        )
-        user = user_handle(sysm.target)
-        if user is None:
-            _lib.check(_lib.load().mb200_leapfrog_euclidean(*args), "mb200_leapfrog_euclidean")
-        else:  # user-written target: general-dimension kernel of its run-time compiled image
-            _lib.check(_lib.load().mb200_leapfrog_euclidean_user(*args, user),
-                       "mb200_leapfrog_euclidean_user")
+            _lib.ptr(status), _lib.ptr(n_done), _lib.current_stream_ptr(dev), target=sysm.target)
 
 
 def _step_args(step_size, n_steps, n, dev):
@@ -319,32 +310,32 @@ def _launch_gaussian(system, step_size, pos, mom, pos_out, mom_out, dirs, n_step
     if eps_t is not None and system.metric.kind == 2:
         raise NotImplementedError("per-chain step sizes with a dense Gaussian-split metric")
     rot = system.rotation_device(dev, eps, drift)
-    rc = _lib.load().mb200_leapfrog_gaussian_euclidean(
-        _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs), n,
-        dim, eps, _lib.ptr(eps_t), n_steps, n_flows, coefs, 1 if initial_h1_flow_step else 0,
-        system.metric.kind, _lib.ptr(system.metric.inv_device(dev)), _lib.ptr(rot),
-        ctypes.byref(model), _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done),
-        _lib.current_stream_ptr(dev),
-    )
-    _lib.check(rc, "mb200_leapfrog_gaussian_euclidean")
+    _lib.call(
+        "mb200_leapfrog_gaussian_euclidean", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out),
+        _lib.ptr(mom_out), _lib.ptr(dirs), n, dim, eps, _lib.ptr(eps_t), n_steps, n_flows, coefs,
+        1 if initial_h1_flow_step else 0, system.metric.kind,
+        _lib.ptr(system.metric.inv_device(dev)), _lib.ptr(rot), ctypes.byref(model), _lib.ptr(h),
+        _lib.ptr(status), _lib.ptr(n_done), _lib.current_stream_ptr(dev))
 
 
 def _gaussian_flow(system, state, dt):
     """In-place ``h2_flow`` of a Gaussian-split system: a one-flow schedule {drift 1.0}."""
-    pos, mom, _, single = _batched(state)
-    pos, mom = pos.contiguous(), mom.contiguous()
-    n = pos.shape[0]
-    pos_out, mom_out = torch.empty_like(pos), torch.empty_like(mom)
-    if isinstance(dt, torch.Tensor) and dt.ndim == 1:
-        dirs = torch.where(dt < 0, -1, 1).to(torch.int32)
-        eps = dt.abs()
-    else:
-        dirs = None if float(dt) >= 0 else torch.full((n,), -1, dtype=torch.int32, device=pos.device)
-        eps = abs(float(dt))
-    _launch_gaussian(system, eps, pos, mom, pos_out, mom_out, dirs, 1, None, None, None,
-                     coefficients=[1.0], initial_h1_flow_step=False)
-    state.pos = _like_input(state.pos, pos_out[0] if single else pos_out)
-    state.mom = _like_input(state.mom, mom_out[0] if single else mom_out)
+
+    def launch(pos, mom, _):
+        n = pos.shape[0]
+        pos_out, mom_out = torch.empty_like(pos), torch.empty_like(mom)
+        if isinstance(dt, torch.Tensor) and dt.ndim == 1:
+            dirs = torch.where(dt < 0, -1, 1).to(torch.int32)
+            eps = dt.abs()
+        else:
+            dirs = None if float(dt) >= 0 else torch.full((n,), -1, dtype=torch.int32,
+                                                          device=pos.device)
+            eps = abs(float(dt))
+        _launch_gaussian(system, eps, pos, mom, pos_out, mom_out, dirs, 1, None, None, None,
+                         coefficients=[1.0], initial_h1_flow_step=False)
+        return pos_out, mom_out
+
+    state.pos, state.mom = _on_batch(state, launch)
 
 
 def _is_per_chain(step_size, n_steps):
@@ -370,8 +361,7 @@ class LeapfrogIntegrator(TractableFlowIntegrator):
     def _host_fast_path(self, pos, mom, dir, out_pos, out_mom, out_status, n_steps, dev,  # noqa: A002
                         n_chunks):
         tensors = (pos, mom, out_pos, out_mom)
-        if (isinstance(self.system, GaussianEuclideanMetricSystem)
-                or isinstance(self.system.target, CudaTarget)
+        if (not _registry_euclidean(self.system)
                 or _is_per_chain(self.step_size, n_steps) or self.step_size is None
                 or any(t.device.type != "cpu" or t.dtype != torch.float64 or not t.is_contiguous()
                        for t in tensors)
@@ -385,31 +375,21 @@ class LeapfrogIntegrator(TractableFlowIntegrator):
             dir_t = dir.to(torch.int32).contiguous()
         elif int(dir) != 1:
             dir_t = torch.full((n,), int(dir), dtype=torch.int32)
-        lib = _lib.load()
         sysm = self.system
-        need = int(lib.mb200_host_scratch_bytes(n, dim))
-        key = ("host_scratch", str(dev))
-        scratch = sysm._dev.get(key)
-        if scratch is None or scratch.numel() < need:
-            scratch = torch.empty(max(need, 8), dtype=torch.uint8, device=dev)
-            sysm._dev[key] = scratch
+        scratch = sysm._scratch("host_scratch", int(_lib.load().mb200_host_scratch_bytes(n, dim)),
+                                dev)
         n_streams = min(n_chunks, 8)
         streams = _host_streams(dev, n_streams)
         handles = (ctypes.c_void_p * n_streams)(*[s.cuda_stream for s in streams])
         model = sysm._model(dev)
         with torch.cuda.device(dev):
             torch.cuda.current_stream(dev).synchronize()  # inputs / scratch of earlier work
-            rc = lib.mb200_leapfrog_euclidean_host(
-                ctypes.c_void_p(pos.data_ptr()), ctypes.c_void_p(mom.data_ptr()),
-                ctypes.c_void_p(out_pos.data_ptr()), ctypes.c_void_p(out_mom.data_ptr()),
-                None if dir_t is None else ctypes.c_void_p(dir_t.data_ptr()), n, dim,
-                float(self.step_size), int(n_steps), sysm.metric.kind,
-                _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model),
-                ctypes.c_void_p(out_status.data_ptr()), n_chunks,
-                ctypes.cast(handles, ctypes.c_void_p), n_streams, _lib.ptr(scratch),
-                scratch.numel(), 1,
-            )
-        _lib.check(rc, "mb200_leapfrog_euclidean_host")
+            _lib.call(
+                "mb200_leapfrog_euclidean_host", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(out_pos),
+                _lib.ptr(out_mom), _lib.ptr(dir_t), n, dim, float(self.step_size), int(n_steps),
+                sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(dev)), ctypes.byref(model),
+                _lib.ptr(out_status), n_chunks, ctypes.cast(handles, ctypes.c_void_p), n_streams,
+                _lib.ptr(scratch), scratch.numel(), 1)
         return True
 
 
@@ -497,15 +477,13 @@ class _ImplicitIntegrator(Integrator):
             ws_args = (_lib.ptr(ws), ws.numel())
         else:
             ws_args = ()
-        rc = getattr(_lib.load(), self._ENTRY)(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), ctypes.byref(model),
+        _lib.call(
+            self._ENTRY, _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out),
+            _lib.ptr(dirs), n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), ctypes.byref(model),
             self.fixed_point_solver.kind, float(kw["convergence_tol"]),
-            float(kw["divergence_tol"]), int(kw["max_iters"]),
-            float(self.reverse_check_tol), _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done),
-            _lib.ptr(iters), *ws_args, _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, self._ENTRY)
+            float(kw["divergence_tol"]), int(kw["max_iters"]), float(self.reverse_check_tol),
+            _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters), *ws_args,
+            _lib.current_stream_ptr(dev))
         return iters
 
 
@@ -553,30 +531,12 @@ class ConstrainedLeapfrogIntegrator(TractableFlowIntegrator):
         self.projection_solver_kwargs = dict(projection_solver_kwargs or {})
 
     def _launch(self, pos, mom, pos_out, mom_out, dirs, n_steps, h, status, n_done):
-        n, dim = pos.shape
+        n = pos.shape[0]
         dev = pos.device
-        sysm = self.system
         kw = self.projection_solver.resolve_kwargs(self.projection_solver_kwargs)
-        model = sysm._model(dev)
         eps, eps_t, ns, max_n = _step_args(self.step_size, n_steps, n, dev)
         iters = torch.zeros(n, dtype=torch.int32, device=dev)
-        metric = (sysm.metric.kind, _lib.ptr(sysm.metric.inv_device(dev)))
-        if isinstance(sysm, GaussianDenseConstrainedEuclideanMetricSystem):
-            # exact h2 rotation with per-chain sin / cos, eigh-inverted Gram matrices
-            entry = "mb200_constrained_leapfrog_gaussian_euclidean"
-            metric += tuple(_lib.ptr(a) for a in sysm.rotation_args(dev))
-        else:
-            entry = "mb200_constrained_leapfrog_euclidean"
-        entry, user = _user_entry(entry, sysm.target)
-        rc = getattr(_lib.load(), entry)(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(dirs),
-            n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), int(self.n_inner_step),
-            *metric, ctypes.byref(model),
-            self.projection_solver.kind, float(kw["constraint_tol"]), float(kw["position_tol"]),
-            float(kw["divergence_tol"]), int(kw["max_iters"]),
-            int(kw.get("max_line_search_iters", 10)), float(self.reverse_check_tol), _lib.ptr(h),
-            _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters), _lib.current_stream_ptr(dev),
-            *user,
-        )
-        _lib.check(rc, entry)
+        self.system._leapfrog(pos, mom, pos_out, mom_out, dirs, eps, eps_t, max_n, ns,
+                              self.n_inner_step, self.projection_solver, kw,
+                              self.reverse_check_tol, h, status, n_done, iters)
         return iters

@@ -279,17 +279,14 @@ def load_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=Fals
     with _lock:
         handle = _handles.get(key)
         if handle is None:
-            lib = _lib.load()
             arr = (ctypes.c_char_p * len(names))(*[n.encode() for n in names])
             handle = ctypes.c_void_p()
             if constraint:
-                rc = lib.mb200_user_constraint_load(cubin, len(cubin), arr, len(names), *constraint,
-                                                    ctypes.byref(handle))
-                _lib.check(rc, "mb200_user_constraint_load")
+                _lib.call("mb200_user_constraint_load", cubin, len(cubin), arr, len(names),
+                          *constraint, ctypes.byref(handle))
             else:
-                rc = lib.mb200_user_target_load(cubin, len(cubin), arr, len(names),
-                                                ctypes.byref(handle))
-                _lib.check(rc, "mb200_user_target_load")
+                _lib.call("mb200_user_target_load", cubin, len(cubin), arr, len(names),
+                          ctypes.byref(handle))
             _handles[key] = handle
         _loaded[(source, name, constraint)] = handle
     return handle

@@ -27,6 +27,7 @@ import torch
 
 from . import _lib
 from .errors import LinAlgError
+from .solvers import solve_projection_onto_manifold_newton
 from .targets import (
     RMETRIC_SOFTABS,
     CudaTarget,
@@ -38,7 +39,6 @@ from .targets import (
     QuadraticScalarMetric,
     Rank1Metric,
     Target,
-    user_handle,
 )
 
 METRIC_IDENTITY, METRIC_DIAGONAL, METRIC_DENSE = 0, 1, 2
@@ -130,7 +130,8 @@ class _FixedMetric:
 
 
 def _batched(state):
-    """View of a state as ([n, D] pos, [n, D] mom, dir tensor-or-None, squeeze flag).
+    """A state as (contiguous [n, D] pos, contiguous [n, D] mom, dir tensor-or-None, squeeze
+    flag).
 
     NumPy arrays (the reference's own ``ChainState`` storage, states.py:160-305) are accepted
     and moved to the current CUDA device; callers convert results back (``_like_input``)."""
@@ -143,7 +144,27 @@ def _batched(state):
     if single:
         pos, mom = pos[None], (None if mom is None else mom[None])
     d = state.dir if "dir" in state else 1
-    return pos, mom, d, single
+    return pos.contiguous(), None if mom is None else mom.contiguous(), d, single
+
+
+def _on_batch(state, launch):
+    """``launch(pos, mom, dir)`` on the batched view of ``state`` (``_batched``); its output
+    tensor, or each tensor of its output tuple, is returned in the form of ``state.pos``: one
+    row for a single chain, NumPy for NumPy."""
+    pos, mom, d, single = _batched(state)
+    out = launch(pos, mom, d)
+
+    def back(x):
+        return _like_input(state.pos, x[0] if single else x)
+
+    return tuple(map(back, out)) if isinstance(out, tuple) else back(out)
+
+
+def _check_metric_status(status, n):
+    """Raise ``LinAlgError`` if the metric of any chain could not be factorised."""
+    if bool((status != 0).any()):
+        bad = int((status != 0).sum())
+        raise LinAlgError(f"metric factorisation failed for {bad} of {n} chains")
 
 
 def _like_input(ref, value):
@@ -193,6 +214,15 @@ class System:
         d = dict(self.__dict__)
         d["_dev"] = {}
         return d
+
+    def _scratch(self, name, nbytes, device):
+        """Device byte buffer ``name`` of at least ``nbytes``, kept and grown across calls."""
+        key = (name, str(device))
+        buf = self._dev.get(key)
+        if buf is None or buf.numel() < nbytes:
+            buf = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=device)
+            self._dev[key] = buf
+        return buf
 
     def _aux_device(self, name, array, device):
         if array is None:
@@ -251,48 +281,34 @@ class EuclideanMetricSystem(TractableFlowSystem):
     def metric(self, value):
         self._metric = value if isinstance(value, _FixedMetric) else _FixedMetric(value)
 
-    def _eval(self, state, *, nld=False, grad=False, vel=False, kin=False):
-        pos, mom, _, single = _batched(state)
-        n, dim = pos.shape
-        dev = pos.device
-        lib = _lib.load()
-        pos = pos.contiguous()
-        mom = pos if mom is None else mom.contiguous()
-        out = {}
-        if nld:
-            out["nld"] = torch.empty(n, dtype=torch.float64, device=dev)
-        if grad:
-            out["grad"] = torch.empty_like(pos)
-        if vel:
-            out["vel"] = torch.empty_like(pos)
-        if kin:
-            out["kin"] = torch.empty(n, dtype=torch.float64, device=dev)
-        user = None
-        if nld or grad:
-            model = self._model(dev)
-            user = user_handle(self.target)
-        else:  # M^-1 p and p.M^-1 p do not involve the target (constrained targets have no
-            model = _lib.Model()  # Euclidean-eval functor): neutral model
-            model.target_id = 0
-        args = (
-            _lib.ptr(pos), _lib.ptr(mom), n, dim, self._metric.kind,
-            _lib.ptr(self._metric.inv_device(dev)), ctypes.byref(model),
-            _lib.ptr(out.get("nld")), _lib.ptr(out.get("grad")), _lib.ptr(out.get("vel")),
-            _lib.ptr(out.get("kin")), _lib.current_stream_ptr(dev),
-        )
-        if user is None:
-            _lib.check(lib.mb200_euclidean_eval(*args), "mb200_euclidean_eval")
-        else:
-            _lib.check(lib.mb200_euclidean_eval_user(*args, user), "mb200_euclidean_eval_user")
-        if single:
-            out = {k: v[0] for k, v in out.items()}
-        return {k: _like_input(state.pos, v) for k, v in out.items()}  # NumPy in -> NumPy out
+    def _eval(self, state, what):
+        """One output of ``mb200_euclidean_eval``: ``"nld"``, ``"grad"``, ``"vel"`` or ``"kin"``."""
+
+        def launch(pos, mom, _):
+            n, dim = pos.shape
+            dev = pos.device
+            mom = pos if mom is None else mom
+            out = torch.empty(n, dtype=torch.float64, device=dev) if what in ("nld", "kin") \
+                else torch.empty_like(pos)
+            target = self.target if what in ("nld", "grad") else None
+            if target is not None:
+                model = self._model(dev)
+            else:  # M^-1 p and p.M^-1 p do not involve the target (constrained targets have no
+                model = _lib.Model()  # Euclidean-eval functor): neutral model
+                model.target_id = 0
+            outs = [_lib.ptr(out) if w == what else None for w in ("nld", "grad", "vel", "kin")]
+            _lib.call("mb200_euclidean_eval", _lib.ptr(pos), _lib.ptr(mom), n, dim,
+                      self._metric.kind, _lib.ptr(self._metric.inv_device(dev)),
+                      ctypes.byref(model), *outs, _lib.current_stream_ptr(dev), target=target)
+            return out
+
+        return _on_batch(state, launch)
 
     def neg_log_dens(self, state):
-        return self._eval(state, nld=True)["nld"]
+        return self._eval(state, "nld")
 
     def grad_neg_log_dens(self, state):
-        return self._eval(state, grad=True)["grad"]
+        return self._eval(state, "grad")
 
     def h1(self, state):
         return self.neg_log_dens(state)
@@ -301,10 +317,10 @@ class EuclideanMetricSystem(TractableFlowSystem):
         return self.grad_neg_log_dens(state)
 
     def h2(self, state):
-        return self._eval(state, kin=True)["kin"]
+        return self._eval(state, "kin")
 
     def dh2_dmom(self, state):
-        return self._eval(state, vel=True)["vel"]
+        return self._eval(state, "vel")
 
     def dh2_dpos(self, state):
         if isinstance(state.pos, np.ndarray):
@@ -316,23 +332,19 @@ class EuclideanMetricSystem(TractableFlowSystem):
 
     def h(self, state):
         """h = h1 + h2 (systems.py:187-196), one fused kernel."""
-        pos, mom, _, single = _batched(state)
-        n, dim = pos.shape
-        dev = pos.device
-        h = torch.empty(n, dtype=torch.float64, device=dev)
-        model = self._model(dev)
-        args = (
-            _lib.ptr(pos.contiguous()), _lib.ptr(mom.contiguous()), n, dim, self._metric.kind,
-            _lib.ptr(self._metric.inv_device(dev)), ctypes.byref(model), _lib.ptr(h),
-            _lib.current_stream_ptr(dev),
-        )
-        user = user_handle(self.target)
-        if user is None:
-            _lib.check(_lib.load().mb200_hamiltonian_euclidean(*args), "mb200_hamiltonian_euclidean")
-        else:
-            _lib.check(_lib.load().mb200_hamiltonian_euclidean_user(*args, user),
-                       "mb200_hamiltonian_euclidean_user")
-        return _like_input(state.pos, h[0] if single else h)
+
+        def launch(pos, mom, _):
+            n, dim = pos.shape
+            dev = pos.device
+            h = torch.empty(n, dtype=torch.float64, device=dev)
+            model = self._model(dev)
+            _lib.call("mb200_hamiltonian_euclidean", _lib.ptr(pos), _lib.ptr(mom), n, dim,
+                      self._metric.kind, _lib.ptr(self._metric.inv_device(dev)),
+                      ctypes.byref(model), _lib.ptr(h), _lib.current_stream_ptr(dev),
+                      target=self.target)
+            return h
+
+        return _on_batch(state, launch)
 
     def h1_flow(self, state, dt):
         """p -= dt * grad l(q) (systems.py:143-152); ``dt`` scalar or per-chain tensor."""
@@ -364,12 +376,9 @@ class EuclideanMetricSystem(TractableFlowSystem):
                 m._dev[key] = torch.as_tensor(fac, device=z.device).contiguous()
             model = _lib.Model()  # the product L z does not involve the target
             model.target_id = 0
-            rc = _lib.load().mb200_euclidean_eval(
-                _lib.ptr(z), _lib.ptr(z), n, dim, m.kind, _lib.ptr(m._dev[key]),
-                ctypes.byref(model), None, None, _lib.ptr(out), None,
-                _lib.current_stream_ptr(z.device),
-            )
-            _lib.check(rc, "mb200_euclidean_eval")
+            _lib.call("mb200_euclidean_eval", _lib.ptr(z), _lib.ptr(z), n, dim, m.kind,
+                      _lib.ptr(m._dev[key]), ctypes.byref(model), None, None, _lib.ptr(out), None,
+                      _lib.current_stream_ptr(z.device))
             z = out
         return _like_input(state.pos, z if state.pos.ndim == 2 else z[0])
 
@@ -440,11 +449,14 @@ class GaussianEuclideanMetricSystem(EuclideanMetricSystem):
         _gaussian_flow(self, state, dt)
 
 
-def _user_entry(entry, target):
-    """``(entry point, trailing arguments)`` of a constrained operation: the ``_user`` twin with
-    the loaded image for a ``CudaTarget``, else the registry entry point with none."""
-    user = user_handle(target)
-    return (entry, ()) if user is None else (entry + "_user", (user,))
+def _registry_euclidean(system):
+    """Whether ``system`` is a plain ``EuclideanMetricSystem`` (not constrained, not a Gaussian
+    split) on a registry target: the systems the tensor-core leapfrog's host-buffer path and the
+    fused dynamic transition serve."""
+    return (isinstance(system, EuclideanMetricSystem)
+            and not isinstance(system, (ConstrainedEuclideanMetricSystem,
+                                        GaussianEuclideanMetricSystem))
+            and not isinstance(system.target, CudaTarget))
 
 
 def _col(dt):
@@ -497,33 +509,49 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
             raise ValueError(f"Target {neg_log_dens!r} defines no constraint function.")
         self.dens_wrt_hausdorff = bool(dens_wrt_hausdorff)
 
-    def h(self, state):
-        """``l(q) + p.M^-1 p/2`` (``dens_wrt_hausdorff=True``: systems.py:842-851, 187-196),
-        evaluated by a zero-step launch of the constrained kernel."""
-        pos, mom, _, single = _batched(state)
+    def _leapfrog(self, pos, mom, pos_out, mom_out, dirs, eps, eps_t, max_n, ns, n_inner_step,
+                  solver, solver_kw, reverse_check_tol, h, status, n_done, iters):
+        """``mb200_constrained_leapfrog[_gaussian]_euclidean`` for this system, with the solver
+        options ``solver_kw`` resolved; ``max_n = 0`` evaluates ``h`` only."""
         n, dim = pos.shape
         dev = pos.device
-        pos, mom = pos.contiguous(), mom.contiguous()
-        h = torch.empty(n, dtype=torch.float64, device=dev)
-        scratch_q, scratch_p = torch.empty_like(pos), torch.empty_like(mom)
         m = self._metric
+        metric = (m.kind, _lib.ptr(m.inv_device(dev)))
+        entry = "mb200_constrained_leapfrog_euclidean"
+        if isinstance(self, GaussianDenseConstrainedEuclideanMetricSystem):
+            # exact h2 rotation with per-chain sin / cos, eigh-inverted Gram matrices
+            entry = "mb200_constrained_leapfrog_gaussian_euclidean"
+            metric += tuple(_lib.ptr(a) for a in self.rotation_args(dev))
         model = self._model(dev)
-        entry, user = _user_entry("mb200_constrained_leapfrog_euclidean", self.target)
-        rc = getattr(_lib.load(), entry)(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(scratch_q), _lib.ptr(scratch_p), None, n, dim,
-            0.0, None, 0, None, 1, m.kind, _lib.ptr(m.inv_device(dev)), ctypes.byref(model), 0,
-            1e-9, 1e-8, 1e10, 50, 10, 2e-8, _lib.ptr(h), None, None, None,
-            _lib.current_stream_ptr(dev), *user,
-        )
-        _lib.check(rc, entry)
-        return _like_input(state.pos, h[0] if single else h)
+        _lib.call(
+            entry, _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out),
+            _lib.ptr(dirs), n, dim, eps, _lib.ptr(eps_t), max_n, _lib.ptr(ns), int(n_inner_step),
+            *metric, ctypes.byref(model), solver.kind, float(solver_kw["constraint_tol"]),
+            float(solver_kw["position_tol"]), float(solver_kw["divergence_tol"]),
+            int(solver_kw["max_iters"]), int(solver_kw.get("max_line_search_iters", 10)),
+            float(reverse_check_tol), _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done),
+            _lib.ptr(iters), _lib.current_stream_ptr(dev), target=self.target)
+
+    def h(self, state):
+        """``h1 + h2`` (systems.py:187-196, 451-454, 842-856), evaluated by a zero-step launch of
+        the constrained kernel."""
+
+        def launch(pos, mom, _):
+            h = torch.empty(pos.shape[0], dtype=torch.float64, device=pos.device)
+            solver = solve_projection_onto_manifold_newton
+            # 2e-8: ConstrainedLeapfrogIntegrator's default reverse_check_tol
+            self._leapfrog(pos, mom, torch.empty_like(pos), torch.empty_like(mom), None, 0.0, None,
+                           0, None, 1, solver, solver.resolve_kwargs({}), 2e-8, h, None, None,
+                           None)
+            return h
+
+        return _on_batch(state, launch)
 
     def project_onto_cotangent_space(self, mom, state):
         """``mom - J^T (J M^-1 J^T)^-1 J M^-1 mom`` at ``state.pos`` (systems.py:863-873) for all
-        chains in one launch (``mb200_project_onto_cotangent_space``)."""
-        return self._project(mom, state, "mb200_project_onto_cotangent_space")
-
-    def _project(self, mom, state, entry):
+        chains in one launch (``mb200_project_onto_cotangent_space``); on the Gaussian system
+        ``J M^-1 J^T`` is inverted through its eigendecomposition (systems.py:1157-1169,
+        ``mb200_project_onto_cotangent_space_gaussian``)."""
         pos = state.pos
         single = pos.ndim == 1
         ref = mom
@@ -539,12 +567,11 @@ class ConstrainedEuclideanMetricSystem(ConstrainedTractableFlowSystem, Euclidean
         m = self._metric
         minv = None if m.kind == METRIC_IDENTITY else m.inv_device(dev)
         model = self._model(dev)
-        entry, user = _user_entry(entry, self.target)
-        rc = getattr(_lib.load(), entry)(
-            _lib.ptr(pos_t), _lib.ptr(mom_t), _lib.ptr(out), n, dim, m.kind, _lib.ptr(minv),
-            ctypes.byref(model), _lib.current_stream_ptr(dev), *user,
-        )
-        _lib.check(rc, entry)
+        gaussian = isinstance(self, GaussianDenseConstrainedEuclideanMetricSystem)
+        _lib.call("mb200_project_onto_cotangent_space" + ("_gaussian" if gaussian else ""),
+                  _lib.ptr(pos_t), _lib.ptr(mom_t), _lib.ptr(out), n, dim, m.kind,
+                  _lib.ptr(minv), ctypes.byref(model), _lib.current_stream_ptr(dev),
+                  target=self.target)
         return _like_input(ref, out[0] if single else out)
 
 
@@ -600,26 +627,8 @@ class GaussianDenseConstrainedEuclideanMetricSystem(GaussianEuclideanMetricSyste
                 for a in (omega, u, None if u is None else u.T))
         return m._dev[key]
 
-    def h(self, state):
-        """``h1 + h2`` (systems.py:187-196, 451-454, 853-856), evaluated by a zero-step launch of
-        the Gaussian constrained kernel."""
-        pos, mom, _, single = _batched(state)
-        n, dim = pos.shape
-        dev = pos.device
-        pos, mom = pos.contiguous(), mom.contiguous()
-        h = torch.empty(n, dtype=torch.float64, device=dev)
-        scratch_q, scratch_p = torch.empty_like(pos), torch.empty_like(mom)
-        m = self._metric
-        om, u, ut = self.rotation_args(dev)
-        entry, user = _user_entry("mb200_constrained_leapfrog_gaussian_euclidean", self.target)
-        rc = getattr(_lib.load(), entry)(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(scratch_q), _lib.ptr(scratch_p), None, n, dim,
-            0.0, None, 0, None, 1, m.kind, _lib.ptr(m.inv_device(dev)), _lib.ptr(om), _lib.ptr(u),
-            _lib.ptr(ut), ctypes.byref(self._model(dev)), 0, 1e-9, 1e-8, 1e10, 50, 10, 2e-8,
-            _lib.ptr(h), None, None, None, _lib.current_stream_ptr(dev), *user,
-        )
-        _lib.check(rc, entry)
-        return _like_input(state.pos, h[0] if single else h)
+    # GaussianEuclideanMetricSystem's h1 + h2 comes first in the MRO
+    h = ConstrainedEuclideanMetricSystem.h
 
     def h2(self, state):
         """``q.q/2 + p.M^-1 p/2`` (systems.py:451-454)."""
@@ -634,12 +643,6 @@ class GaussianDenseConstrainedEuclideanMetricSystem(GaussianEuclideanMetricSyste
             "The exact h2 flow of a constrained Gaussian system runs inside the constrained "
             "leapfrog kernel, followed by the projection onto the manifold.")
 
-    def project_onto_cotangent_space(self, mom, state):
-        """``mom - J^T gram^-1 (J M^-1 mom)`` with ``gram`` a ``DenseSymmetricMatrix`` inverted
-        through its eigendecomposition (systems.py:863-873, 1157-1169), all chains in one launch
-        (``mb200_project_onto_cotangent_space_gaussian``)."""
-        return self._project(mom, state, "mb200_project_onto_cotangent_space_gaussian")
-
 
 class RiemannianMetricSystem(System):
     """Riemannian Hamiltonian system with a position-dependent metric (systems.py:1187-1402)."""
@@ -647,54 +650,45 @@ class RiemannianMetricSystem(System):
     def _workspace(self, n, dim, device):
         model = self._model(device)
         nbytes = int(_lib.load().mb200_implicit_workspace_bytes(n, dim, ctypes.byref(model)))
-        key = ("ws", str(device))
-        ws = self._dev.get(key)
-        if ws is None or ws.numel() < nbytes:
-            ws = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=device)
-            self._dev[key] = ws
-        return ws
+        return self._scratch("ws", nbytes, device)
 
     def h(self, state):
         """l(q) + log|M(q)|/2 + p^T M(q)^-1 p / 2 (systems.py:1375-1390)."""
-        pos, mom, _, single = _batched(state)
-        n, dim = pos.shape
-        dev = pos.device
-        h = torch.empty(n, dtype=torch.float64, device=dev)
-        status = torch.empty(n, dtype=torch.int32, device=dev)
-        ws = self._workspace(n, dim, dev)
-        model = self._model(dev)
-        rc = _lib.load().mb200_hamiltonian_riemannian(
-            _lib.ptr(pos.contiguous()), _lib.ptr(mom.contiguous()), n, dim, ctypes.byref(model),
-            _lib.ptr(h), _lib.ptr(status), _lib.ptr(ws), ws.numel(), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_hamiltonian_riemannian")
-        return _like_input(state.pos, h[0] if single else h)
+
+        def launch(pos, mom, _):
+            n, dim = pos.shape
+            dev = pos.device
+            h = torch.empty(n, dtype=torch.float64, device=dev)
+            status = torch.empty(n, dtype=torch.int32, device=dev)
+            ws = self._workspace(n, dim, dev)
+            model = self._model(dev)
+            _lib.call("mb200_hamiltonian_riemannian", _lib.ptr(pos), _lib.ptr(mom), n, dim,
+                      ctypes.byref(model), _lib.ptr(h), _lib.ptr(status), _lib.ptr(ws),
+                      ws.numel(), _lib.current_stream_ptr(dev))
+            return h
+
+        return _on_batch(state, launch)
 
     def dh2_dmom(self, state):
         """``M(q)^-1 p`` (systems.py:1398-1399); not cached, as in the reference."""
-        from .errors import LinAlgError  # noqa: PLC0415
 
-        pos, mom, _, single = _batched(state)
-        n, dim = pos.shape
-        dev = pos.device
-        vel = torch.empty((n, dim), dtype=torch.float64, device=dev)
-        status = torch.empty(n, dtype=torch.int32, device=dev)
-        model = self._model(dev)
-        rc = _lib.load().mb200_dh_dmom_riemannian(
-            _lib.ptr(pos.contiguous()), _lib.ptr(mom.contiguous()), _lib.ptr(vel), n, dim,
-            ctypes.byref(model), _lib.ptr(status), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_dh_dmom_riemannian")
-        if bool((status != 0).any()):
-            bad = int((status != 0).sum())
-            raise LinAlgError(f"metric factorisation failed for {bad} of {n} chains")
-        return _like_input(state.pos, vel[0] if single else vel)
+        def launch(pos, mom, _):
+            n, dim = pos.shape
+            dev = pos.device
+            vel = torch.empty((n, dim), dtype=torch.float64, device=dev)
+            status = torch.empty(n, dtype=torch.int32, device=dev)
+            model = self._model(dev)
+            _lib.call("mb200_dh_dmom_riemannian", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(vel), n,
+                      dim, ctypes.byref(model), _lib.ptr(status), _lib.current_stream_ptr(dev))
+            _check_metric_status(status, n)
+            return vel
+
+        return _on_batch(state, launch)
 
     def sample_momentum(self, state, rng):
         """``metric(state).sqrt @ N(0, I)`` (systems.py:1401-1402): the factor of M(q) is built
         per chain on the device (``mb200_sample_momentum_riemannian``).  Chains whose metric
         cannot be built raise ``LinAlgError`` as in the reference."""
-        from .errors import LinAlgError  # noqa: PLC0415
         from .transitions import _normals  # noqa: PLC0415
 
         pos = torch.as_tensor(state.pos)
@@ -708,14 +702,9 @@ class RiemannianMetricSystem(System):
         out = torch.empty_like(z)
         status = torch.empty(n, dtype=torch.int32, device=dev)
         model = self._model(dev)
-        rc = _lib.load().mb200_sample_momentum_riemannian(
-            _lib.ptr(pos), _lib.ptr(z), _lib.ptr(out), n, dim, ctypes.byref(model),
-            _lib.ptr(status), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_sample_momentum_riemannian")
-        if bool((status != 0).any()):
-            bad = int((status != 0).sum())
-            raise LinAlgError(f"metric factorisation failed for {bad} of {n} chains")
+        _lib.call("mb200_sample_momentum_riemannian", _lib.ptr(pos), _lib.ptr(z), _lib.ptr(out),
+                  n, dim, ctypes.byref(model), _lib.ptr(status), _lib.current_stream_ptr(dev))
+        _check_metric_status(status, n)
         return _like_input(state.pos, out[0] if single else out)
 
 

@@ -31,7 +31,7 @@ import torch
 
 from . import _lib
 from .states import ChainState
-from .systems import _dir_tensor
+from .systems import _dir_tensor, _registry_euclidean
 
 
 def _normals(rng, shape, device):
@@ -42,6 +42,29 @@ def _normals(rng, shape, device):
     else:
         z = rng.standard_normal(shape)
     return torch.as_tensor(z, device=device)
+
+
+def _uniform_table(rng, n, n_uniforms, device):
+    """The ``[n, n_uniforms]`` uniforms of one dynamic transition, and the state of each per-chain
+    generator before the draw (``None`` unless ``rng`` is a sequence of generators)."""
+    if isinstance(rng, torch.Generator):
+        return torch.rand((n, n_uniforms), dtype=torch.float64, device=device, generator=rng), None
+    if isinstance(rng, Sequence):
+        saved = [g.bit_generator.state for g in rng]
+        return torch.as_tensor(np.stack([g.uniform(size=n_uniforms) for g in rng]),
+                               device=device), saved
+    return torch.as_tensor(rng.uniform(size=(n, n_uniforms)), device=device), None
+
+
+def _replay(rng, saved, used):
+    """Leave every chain's generator advanced by exactly the ``used`` uniforms its chain
+    consumed."""
+    if saved is None:
+        return
+    for g, st, k in zip(rng, saved, used.cpu().tolist()):
+        g.bit_generator.state = st
+        if k:
+            g.uniform(size=k)
 
 
 def _uniforms(rng, n, device, mask=None):
@@ -135,13 +158,10 @@ class MetropolisIntegrationTransition:
         accept_prob = torch.empty(n, dtype=torch.float64, device=dev)
         accept_stat = torch.empty(n, dtype=torch.float64, device=dev)
         accepted = torch.empty(n, dtype=torch.int32, device=dev)
-        rc = _lib.load().mb200_metropolis_select(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(prop.pos), _lib.ptr(prop.mom),
-            _lib.ptr(h_init), _lib.ptr(prop.h), _lib.ptr(status), _lib.ptr(n_done),
-            _lib.ptr(dirs), _lib.ptr(u), n, dim, _lib.ptr(accept_prob), _lib.ptr(accept_stat),
-            _lib.ptr(accepted), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_metropolis_select")
+        _lib.call("mb200_metropolis_select", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(prop.pos),
+                  _lib.ptr(prop.mom), _lib.ptr(h_init), _lib.ptr(prop.h), _lib.ptr(status),
+                  _lib.ptr(n_done), _lib.ptr(dirs), _lib.ptr(u), n, dim, _lib.ptr(accept_prob),
+                  _lib.ptr(accept_stat), _lib.ptr(accepted), _lib.current_stream_ptr(dev))
         new = ChainState(pos=pos, mom=mom, dir=dirs)
         stats = {
             "n_step": n_done.to(torch.int64),
@@ -231,12 +251,6 @@ class DynamicIntegrationTransition:
                  termination_criterion=riemannian_no_u_turn_criterion,
                  do_extra_subtree_checks=True):
         from .integrators import LeapfrogIntegrator  # noqa: PLC0415
-        from .targets import CudaTarget  # noqa: PLC0415
-        from .systems import (  # noqa: PLC0415
-            ConstrainedEuclideanMetricSystem,
-            EuclideanMetricSystem,
-            GaussianEuclideanMetricSystem,
-        )
 
         if self._slice is None:
             raise TypeError("Use MultinomialDynamicIntegrationTransition or "
@@ -250,10 +264,7 @@ class DynamicIntegrationTransition:
         # (mb200_nuts_euclidean).  Every other pair (constrained, implicit, compositions,
         # Gaussian splitting, user-written targets): lock-step leaves through the integrator's own
         # kernels with the tree bookkeeping in the mb200_nuts_generic_* kernels.
-        self._fused = type(integrator) is LeapfrogIntegrator and isinstance(
-            system, EuclideanMetricSystem) and not isinstance(
-            system, (ConstrainedEuclideanMetricSystem, GaussianEuclideanMetricSystem)) \
-            and not isinstance(system.target, CudaTarget)
+        self._fused = type(integrator) is LeapfrogIntegrator and _registry_euclidean(system)
         self.system = system
         self.integrator = integrator
         self.max_tree_depth = int(max_tree_depth)
@@ -277,22 +288,11 @@ class DynamicIntegrationTransition:
         n, dim = pos.shape
         dev = pos.device
         n_uni = self.n_uniforms
-        saved = None
-        if isinstance(rng, torch.Generator):
-            uni = torch.rand((n, n_uni), dtype=torch.float64, device=dev, generator=rng)
-        elif isinstance(rng, Sequence):
-            saved = [g.bit_generator.state for g in rng]
-            uni = torch.as_tensor(np.stack([g.uniform(size=n_uni) for g in rng]), device=dev)
-        else:
-            uni = torch.as_tensor(rng.uniform(size=(n, n_uni)), device=dev)
-        lib = _lib.load()
-        nbytes = int(lib.mb200_nuts_workspace_bytes(n, dim, self.max_tree_depth))
+        uni, saved = _uniform_table(rng, n, n_uni, dev)
+        nbytes = int(_lib.load().mb200_nuts_workspace_bytes(n, dim, self.max_tree_depth))
         if nbytes < 0:
             raise ValueError("unsupported dim / max_tree_depth for the fused dynamic transition")
-        ws = self.system._dev.get(("nuts_ws", str(dev)))
-        if ws is None or ws.numel() < nbytes:
-            ws = torch.empty(max(nbytes, 8), dtype=torch.uint8, device=dev)
-            self.system._dev[("nuts_ws", str(dev))] = ws
+        ws = self.system._scratch("nuts_ws", nbytes, dev)
         eps = self.integrator.step_size
         per_chain = isinstance(eps, torch.Tensor) and eps.ndim == 1
         eps_t = eps.to(device=dev, dtype=torch.float64).contiguous() if per_chain else None
@@ -304,40 +304,23 @@ class DynamicIntegrationTransition:
         used, status, dir_out = torch.empty(n, **i32), torch.empty(n, **i32), torch.empty(n, **i32)
         m = self.system.metric
         model = self.system._model(dev)
-        rc = lib.mb200_nuts_euclidean(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out), _lib.ptr(mom_out), n, dim,
-            0.0 if per_chain else float(eps), _lib.ptr(eps_t), m.kind,
+        _lib.call(
+            "mb200_nuts_euclidean", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(pos_out),
+            _lib.ptr(mom_out), n, dim, 0.0 if per_chain else float(eps), _lib.ptr(eps_t), m.kind,
             _lib.ptr(m.inv_device(dev)), ctypes.byref(model), 1 if self._slice else 0,
             1 if self.termination_criterion is euclidean_no_u_turn_criterion else 0,
             1 if self.do_extra_subtree_checks else 0, self.max_tree_depth, self.max_delta_h,
             _lib.ptr(uni), n_uni, _lib.ptr(ws), ws.numel(), _lib.ptr(h), _lib.ptr(n_step),
             _lib.ptr(av), _lib.ptr(rej), _lib.ptr(depth), _lib.ptr(div), _lib.ptr(used),
-            _lib.ptr(dir_out), _lib.ptr(status), _lib.current_stream_ptr(dev),
-        )
-        _lib.check(rc, "mb200_nuts_euclidean")
-        if saved is not None:
-            # leave every chain's generator advanced by exactly what its chain consumed
-            for g, st, k in zip(rng, saved, used.cpu().tolist()):
-                g.bit_generator.state = st
-                if k:
-                    g.uniform(size=k)
+            _lib.ptr(dir_out), _lib.ptr(status), _lib.current_stream_ptr(dev))
+        _replay(rng, saved, used)
         if bool((status != 0).any()):
             raise RuntimeError("dynamic transition ran out of uniform variates")
         diverging = div.bool()
-        new = ChainState(pos=pos_out, mom=mom_out, dir=dir_out)
-        new.h = h
-        stats = {
-            "n_step": n_step.to(torch.int64),
-            "accept_stat": torch.where(diverging, torch.zeros_like(av), av),
-            "av_metrop_accept_prob": av,
-            "reject_prob": rej,
-            "tree_depth": depth.to(torch.int64),
-            "diverging": diverging,
-            "convergence_error": torch.zeros(n, dtype=torch.bool, device=dev),
-            "non_reversible_step": torch.zeros(n, dtype=torch.bool, device=dev),
-            "step_size": _step_size_stat(eps, n, dev),
-        }
-        return new, stats
+        no_failure = {"dtype": torch.bool, "device": dev}
+        return _dynamic_result(pos_out, mom_out, dir_out, h, n_step, av, rej, depth, diverging,
+                               torch.zeros(n, **no_failure), torch.zeros(n, **no_failure),
+                               diverging, eps)
 
     def _sample_generic(self, state, rng):
         """Lock-step dynamic transition through the integrator's own step kernels."""
@@ -345,24 +328,14 @@ class DynamicIntegrationTransition:
         n, dim = pos.shape
         dev = pos.device
         n_uni = self.n_uniforms
-        saved = None
-        if isinstance(rng, torch.Generator):
-            uni = torch.rand((n, n_uni), dtype=torch.float64, device=dev, generator=rng)
-        elif isinstance(rng, Sequence):
-            saved = [g.bit_generator.state for g in rng]
-            uni = torch.as_tensor(np.stack([g.uniform(size=n_uni) for g in rng]), device=dev)
-        else:
-            uni = torch.as_tensor(rng.uniform(size=(n, n_uni)), device=dev)
+        uni, saved = _uniform_table(rng, n, n_uni, dev)
         lib = _lib.load()
         system, integ = self.system, self.integrator
         ws_bytes = int(lib.mb200_nuts_workspace_bytes(n, dim, self.max_tree_depth))
         cs_bytes = int(lib.mb200_nuts_generic_state_bytes(n))
         if ws_bytes < 0:
             raise ValueError("unsupported dim / max_tree_depth for the dynamic transition")
-        ws = system._dev.get(("nuts_ws", str(dev)))
-        if ws is None or ws.numel() < ws_bytes:
-            ws = torch.empty(max(ws_bytes, 8), dtype=torch.uint8, device=dev)
-            system._dev[("nuts_ws", str(dev))] = ws
+        ws = system._scratch("nuts_ws", ws_bytes, dev)
         cs = torch.empty(max(cs_bytes, 8), dtype=torch.uint8, device=dev)
         opts = _lib.NutsOptions()
         opts.max_tree_depth = self.max_tree_depth
@@ -380,15 +353,14 @@ class DynamicIntegrationTransition:
         init = ChainState(pos=pos, mom=mom, dir=1)
         h0 = system.h(init).contiguous()
         v0 = system.dh_dmom(init).contiguous()
-        _lib.check(lib.mb200_nuts_generic_begin(
-            _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(v0), _lib.ptr(h0), n, dim, o, _lib.ptr(ws),
-            ws.numel(), _lib.ptr(cs), cs.numel(), stream), "mb200_nuts_generic_begin")
+        _lib.call("mb200_nuts_generic_begin", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(v0),
+                  _lib.ptr(h0), n, dim, o, _lib.ptr(ws), ws.numel(), _lib.ptr(cs), cs.numel(),
+                  stream)
         q_edge, p_edge = torch.empty_like(pos), torch.empty_like(mom)
         dirs, active = torch.empty(n, **i32), torch.empty(n, **i32)
         for depth in range(self.max_tree_depth):
-            _lib.check(lib.mb200_nuts_generic_start(
-                n, dim, depth, o, _lib.ptr(ws), _lib.ptr(cs), _lib.ptr(q_edge), _lib.ptr(p_edge),
-                _lib.ptr(dirs), _lib.ptr(active), stream), "mb200_nuts_generic_start")
+            _lib.call("mb200_nuts_generic_start", n, dim, depth, o, _lib.ptr(ws), _lib.ptr(cs),
+                      _lib.ptr(q_edge), _lib.ptr(p_edge), _lib.ptr(dirs), _lib.ptr(active), stream)
             if not bool(active.any()):
                 break
             cur = ChainState(pos=q_edge, mom=p_edge, dir=dirs)
@@ -396,49 +368,52 @@ class DynamicIntegrationTransition:
             for k in range(1, n_leaves + 1):
                 new = integ.step_n(cur, 1, return_h=True)
                 vel = system.dh_dmom(_quiet(new)).contiguous()
-                _lib.check(lib.mb200_nuts_generic_leaf(
-                    _lib.ptr(new.pos), _lib.ptr(new.mom), _lib.ptr(vel), _lib.ptr(new.h),
-                    _lib.ptr(new.status), n, dim, k, n_leaves, o, _lib.ptr(ws), _lib.ptr(cs),
-                    _lib.ptr(active), stream), "mb200_nuts_generic_leaf")
+                _lib.call("mb200_nuts_generic_leaf", _lib.ptr(new.pos), _lib.ptr(new.mom),
+                          _lib.ptr(vel), _lib.ptr(new.h), _lib.ptr(new.status), n, dim, k,
+                          n_leaves, o, _lib.ptr(ws), _lib.ptr(cs), _lib.ptr(active), stream)
                 cur = ChainState(pos=new.pos, mom=new.mom, dir=dirs)
                 # every chain's doubling may have terminated early: look now and then
                 if k < n_leaves and (k & 7) == 0 and not bool(active.any()):
                     break
-            _lib.check(lib.mb200_nuts_generic_finish(
-                n, dim, depth, o, _lib.ptr(ws), _lib.ptr(cs), stream), "mb200_nuts_generic_finish")
+            _lib.call("mb200_nuts_generic_finish", n, dim, depth, o, _lib.ptr(ws), _lib.ptr(cs),
+                      stream)
         pos_out, mom_out = torch.empty_like(pos), torch.empty_like(mom)
         h, av, rej = torch.empty(n, **f64), torch.empty(n, **f64), torch.empty(n, **f64)
         n_step, tdepth, flags = torch.empty(n, **i32), torch.empty(n, **i32), torch.empty(n, **i32)
         used, dir_out = torch.empty(n, **i32), torch.empty(n, **i32)
-        _lib.check(lib.mb200_nuts_generic_end(
-            n, dim, o, _lib.ptr(ws), _lib.ptr(cs), _lib.ptr(pos_out), _lib.ptr(mom_out),
-            _lib.ptr(h), _lib.ptr(n_step), _lib.ptr(av), _lib.ptr(rej), _lib.ptr(tdepth),
-            _lib.ptr(flags), _lib.ptr(used), _lib.ptr(dir_out), stream), "mb200_nuts_generic_end")
-        if saved is not None:
-            for g, st, k in zip(rng, saved, used.cpu().tolist()):
-                g.bit_generator.state = st
-                if k:
-                    g.uniform(size=k)
+        _lib.call("mb200_nuts_generic_end", n, dim, o, _lib.ptr(ws), _lib.ptr(cs),
+                  _lib.ptr(pos_out), _lib.ptr(mom_out), _lib.ptr(h), _lib.ptr(n_step), _lib.ptr(av),
+                  _lib.ptr(rej), _lib.ptr(tdepth), _lib.ptr(flags), _lib.ptr(used),
+                  _lib.ptr(dir_out), stream)
+        _replay(rng, saved, used)
         if bool(((flags >> 3) & 1).any()):
             raise RuntimeError("dynamic transition ran out of uniform variates")
         diverging = (flags & 1).bool()
         conv = ((flags >> 1) & 1).bool()
         nonrev = ((flags >> 2) & 1).bool()
-        failed = diverging | conv | nonrev
-        new = ChainState(pos=pos_out, mom=mom_out, dir=dir_out)
-        new.h = h
-        stats = {
-            "n_step": n_step.to(torch.int64),
-            "accept_stat": torch.where(failed, torch.zeros_like(av), av),
-            "av_metrop_accept_prob": av,
-            "reject_prob": rej,
-            "tree_depth": tdepth.to(torch.int64),
-            "diverging": diverging,
-            "convergence_error": conv,
-            "non_reversible_step": nonrev,
-            "step_size": _step_size_stat(integ.step_size, n, dev),
-        }
-        return new, stats
+        return _dynamic_result(pos_out, mom_out, dir_out, h, n_step, av, rej, tdepth, diverging,
+                               conv, nonrev, diverging | conv | nonrev, integ.step_size)
+
+
+def _dynamic_result(pos, mom, dirs, h, n_step, av, rej, depth, diverging, conv, nonrev, failed,
+                    step_size):
+    """The next state and the statistics of a dynamic transition (transitions.py:758-769); a
+    failed chain's ``accept_stat`` is 0."""
+    n = pos.shape[0]
+    new = ChainState(pos=pos, mom=mom, dir=dirs)
+    new.h = h
+    stats = {
+        "n_step": n_step.to(torch.int64),
+        "accept_stat": torch.where(failed, torch.zeros_like(av), av),
+        "av_metrop_accept_prob": av,
+        "reject_prob": rej,
+        "tree_depth": depth.to(torch.int64),
+        "diverging": diverging,
+        "convergence_error": conv,
+        "non_reversible_step": nonrev,
+        "step_size": _step_size_stat(step_size, n, pos.device),
+    }
+    return new, stats
 
 
 def _quiet(state):
