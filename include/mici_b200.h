@@ -95,6 +95,11 @@ extern "C" {
 /* Cholesky-factored metric M = L L^T given by its lower factor (CholeskyFactoredRiemannianMetricSystem,
  * systems.py:1574-1653); targets: std-Gaussian, banana, funnel, quadratic */
 #define MB200_RMETRIC_CHOL_QUADRATIC 6 /* L(q) = L0 + c tril(q q^T);  aux: L0 [dim*dim] row-major, upper triangle zero (never read), params: c */
+/* user-written diagonal / scalar metrics compiled at run time with a user target
+ * (mb200_user_riemannian_load); only the Riemannian *_user entry points accept them, every registry
+ * entry point rejects them as an unknown rmetric_id.  params / aux: the metric's own */
+#define MB200_RMETRIC_USER_DIAGONAL 32
+#define MB200_RMETRIC_USER_SCALAR 33
 
 /* fixed-point solvers fused into the implicit integrators (solvers.py:47-94, 97-154) */
 #define MB200_FP_SOLVER_DIRECT 0
@@ -460,6 +465,51 @@ int mb200_sample_momentum_riemannian(const double* pos, const double* normals, d
 int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_out,
                              int64_t n_chains, int32_t dim, const mb200_model* model,
                              int32_t* status, void* stream);
+
+/*
+ * User-written targets and metrics on the diagonal and scalar Riemannian systems
+ * (mici_b200/csrc/user_riemannian.cuh): a user target and a user diagonal or scalar metric
+ * compiled at run time, by NVRTC, together with the Riemannian kernels of the compact policies.
+ *  - mb200_user_riemannian_load: loads a CUBIN `image` of `n_names` = 3 kernels, with
+ *    T = UserRTarget and M = UserDiagonalMetric (rmetric_id MB200_RMETRIC_USER_DIAGONAL) or
+ *    UserScalarMetric (MB200_RMETRIC_USER_SCALAR): implicit_leapfrog_kernel<T, M>,
+ *    riemannian_velocity_kernel<T, M>, riemannian_sample_momentum_kernel<T, M>.  The handle is
+ *    released by mb200_user_target_unload.  It serves only the Riemannian *_user entry points;
+ *    the Euclidean and constrained ones refuse it, and these refuse every other handle.
+ *  - mb200_implicit_leapfrog_riemannian_user, mb200_implicit_midpoint_riemannian_user,
+ *    mb200_hamiltonian_riemannian_user, mb200_sample_momentum_riemannian_user,
+ *    mb200_dh_dmom_riemannian_user: the contracts of the entry points without `_user`, for
+ *    model->target_id == MB200_TARGET_USER, model->rmetric_id == the handle's rmetric_id and a
+ *    `user_image` from mb200_user_riemannian_load; anything else is MB200_ERR_INVALID_ARG and
+ *    launches nothing.  No workspace is needed (mb200_implicit_workspace_bytes returns 0).
+ */
+int mb200_user_riemannian_load(const void* image, int64_t image_bytes, const char* const* names,
+                               int32_t n_names, int32_t rmetric_id, void** handle);
+int mb200_implicit_leapfrog_riemannian_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* workspace, int64_t workspace_bytes, void* stream, const void* user_image);
+int mb200_implicit_midpoint_riemannian_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* stream, const void* user_image);
+int mb200_hamiltonian_riemannian_user(const double* pos, const double* mom, int64_t n_chains,
+                                      int32_t dim, const mb200_model* model, double* h_out,
+                                      int32_t* status, void* workspace, int64_t workspace_bytes,
+                                      void* stream, const void* user_image);
+int mb200_sample_momentum_riemannian_user(const double* pos, const double* normals,
+                                          double* mom_out, int64_t n_chains, int32_t dim,
+                                          const mb200_model* model, int32_t* status, void* stream,
+                                          const void* user_image);
+int mb200_dh_dmom_riemannian_user(const double* pos, const double* mom, double* vel_out,
+                                  int64_t n_chains, int32_t dim, const mb200_model* model,
+                                  int32_t* status, void* stream, const void* user_image);
 
 /*
  * "Next" row N4: GaussianEuclideanMetricSystem (systems.py:369-474) -- the target density is

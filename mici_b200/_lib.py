@@ -137,13 +137,17 @@ SIGNATURES = {
         [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _I64, _I32, _P, _P, _P, _P],
     ),
     "mb200_hamiltonian_riemannian": (ctypes.c_int, [_P, _P, _I64, _I32, _MP, _P, _P, _P, _I64, _P]),
+    "mb200_user_riemannian_load": (ctypes.c_int, [ctypes.c_char_p, _I64, _P, _I32, _I32, _P]),
 }
 
 # each `_user` twin takes its registry entry point's arguments plus the loaded image's handle
 for _name in ("mb200_leapfrog_euclidean", "mb200_hamiltonian_euclidean", "mb200_euclidean_eval",
               "mb200_constrained_leapfrog_euclidean",
               "mb200_constrained_leapfrog_gaussian_euclidean",
-              "mb200_project_onto_cotangent_space", "mb200_project_onto_cotangent_space_gaussian"):
+              "mb200_project_onto_cotangent_space", "mb200_project_onto_cotangent_space_gaussian",
+              "mb200_implicit_leapfrog_riemannian", "mb200_implicit_midpoint_riemannian",
+              "mb200_hamiltonian_riemannian", "mb200_sample_momentum_riemannian",
+              "mb200_dh_dmom_riemannian"):
     SIGNATURES[_name + "_user"] = (SIGNATURES[_name][0], SIGNATURES[_name][1] + [_P])
 
 _lock = threading.Lock()
@@ -176,8 +180,9 @@ def load():
 
 
 def call(entry, *args, target=None):
-    """Call the entry point ``entry`` and raise if it fails.  For a user-written ``CudaTarget``
-    it calls the ``_user`` twin instead, with the target's loaded image appended."""
+    """Call the entry point ``entry`` and raise if it fails.  For a user-written ``CudaTarget``,
+    or a ``CudaTarget`` paired with a user metric, it calls the ``_user`` twin instead, with the
+    loaded image appended."""
     from .targets import user_handle  # noqa: PLC0415
 
     user = user_handle(target)

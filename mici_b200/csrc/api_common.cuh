@@ -252,6 +252,19 @@ struct UserConstraintKernels {
 // the constrained part of a loaded user image (api_euclid.cu)
 const UserConstraintKernels& user_constraint_kernels(const void* handle);
 
+// The Riemannian kernels of a user image loaded by mb200_user_riemannian_load, for one (user
+// target, user metric) pair: the implicit leapfrog / midpoint, velocity and momentum-refresh
+// kernels of the metric kind rmetric_id.  rmetric_id == 0: an image of mb200_user_target_load or
+// mb200_user_constraint_load, which carries none (and whose Euclidean kernels this one lacks).
+struct UserRiemannianKernels {
+  int rmetric_id;
+  const void* implicit;
+  const void* velocity;
+  const void* momentum;
+};
+// the Riemannian part of a loaded user image (api_euclid.cu)
+const UserRiemannianKernels& user_riemannian_kernels(const void* handle);
+
 // Arguments of one implicit-integrator launch on a Riemannian system (leapfrog or midpoint steps;
 // zero steps evaluate the Hamiltonian only).  ws / ws_bytes: the caller's workspace, or NULL.
 struct ImplicitArgs {

@@ -109,6 +109,7 @@ using LeapfrogKernel = decltype(&leapfrog_generic_kernel<StdGaussianTarget, 1, 4
 using EvalKernel = decltype(&euclidean_eval_kernel<StdGaussianTarget, 1>);
 struct UserKernels {
   cudaLibrary_t lib;
+  UserRiemannianKernels rm;  // mb200_user_riemannian_load only, which has no other kernels
   LeapfrogKernel leapfrog[N_EU_LAYOUTS];
   EvalKernel eval[N_EU_LAYOUTS];
   UserConstraintKernels constr;  // mb200_user_constraint_load only
@@ -118,12 +119,29 @@ const UserConstraintKernels& user_constraint_kernels(const void* handle) {
   return static_cast<const UserKernels*>(handle)->constr;
 }
 
+const UserRiemannianKernels& user_riemannian_kernels(const void* handle) {
+  return static_cast<const UserKernels*>(handle)->rm;
+}
+
+// The handle of a Euclidean *_user entry point: an image with the Euclidean kernels
+static int euclidean_image(const void* handle, const UserKernels** u) {
+  if (!handle) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  *u = static_cast<const UserKernels*>(handle);
+  if ((*u)->rm.rmetric_id != 0)
+    return fail(MB200_ERR_INVALID_ARG,
+                "a Riemannian user image (mb200_user_riemannian_load) has no Euclidean kernels");
+  return 0;
+}
+
 // Loads `image` and looks up its kernels: the Euclidean table, then (n_names > 2 N_EU_LAYOUTS)
-// the constrained one, in the order of include/mici_b200.h
+// the constrained one, in the order of include/mici_b200.h; or, for an image of
+// mb200_user_riemannian_load (rm.rmetric_id != 0), its three Riemannian kernels only
 static int user_image_load(const void* image, const char* const* names, int n_names,
-                           const UserConstraintKernels& constr, void** handle) {
+                           const UserConstraintKernels& constr, const UserRiemannianKernels& rm,
+                           void** handle) {
   UserKernels* u = new UserKernels();
   u->constr = constr;
+  u->rm = rm;
   cudaError_t e = cudaLibraryLoadData(&u->lib, image, nullptr, nullptr, 0, nullptr, nullptr, 0);
   if (e != cudaSuccess) {
     delete u;
@@ -138,7 +156,10 @@ static int user_image_load(const void* image, const char* const* names, int n_na
       return fail(MB200_ERR_CUDA, "cudaLibraryGetKernel(%s): %s", names[i], cudaGetErrorString(e));
     }
     const int c = i - 2 * N_EU_LAYOUTS;
-    if (i < N_EU_LAYOUTS)
+    if (rm.rmetric_id != 0)
+      (i == 0 ? u->rm.implicit : i == 1 ? u->rm.velocity : u->rm.momentum) =
+          reinterpret_cast<const void*>(k);
+    else if (i < N_EU_LAYOUTS)
       u->leapfrog[i] = reinterpret_cast<LeapfrogKernel>(k);
     else if (c < 0)
       u->eval[i - N_EU_LAYOUTS] = reinterpret_cast<EvalKernel>(k);
@@ -371,7 +392,8 @@ int mb200_user_target_load(const void* image, int64_t image_bytes, const char* c
   if (n_names != 2 * N_EU_LAYOUTS)
     return fail(MB200_ERR_INVALID_ARG, "expected %d kernel names, got %d", 2 * N_EU_LAYOUTS,
                 n_names);
-  return user_image_load(image, names, n_names, UserConstraintKernels{}, handle);
+  return user_image_load(image, names, n_names, UserConstraintKernels{}, UserRiemannianKernels{},
+                         handle);
 }
 
 int mb200_user_constraint_load(const void* image, int64_t image_bytes, const char* const* names,
@@ -385,7 +407,20 @@ int mb200_user_constraint_load(const void* image, int64_t image_bytes, const cha
   if (n_constr < 1 || n_constr > 8 || (kp != 1 && kp != 2 && kp != 4))
     return fail(MB200_ERR_INVALID_ARG, "n_constr must be in [1, 8] and kp 1, 2 or 4");
   return user_image_load(image, names, n_names,
-                         UserConstraintKernels{n_constr, kp, mhp_constr != 0, {}, {}}, handle);
+                         UserConstraintKernels{n_constr, kp, mhp_constr != 0, {}, {}},
+                         UserRiemannianKernels{}, handle);
+}
+
+int mb200_user_riemannian_load(const void* image, int64_t image_bytes, const char* const* names,
+                               int32_t n_names, int32_t rmetric_id, void** handle) {
+  if (!image || image_bytes <= 0 || !names || !handle)
+    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_names != 3) return fail(MB200_ERR_INVALID_ARG, "expected 3 kernel names, got %d", n_names);
+  if (rmetric_id != MB200_RMETRIC_USER_DIAGONAL && rmetric_id != MB200_RMETRIC_USER_SCALAR)
+    return fail(MB200_ERR_INVALID_ARG,
+                "rmetric_id must be MB200_RMETRIC_USER_DIAGONAL or MB200_RMETRIC_USER_SCALAR");
+  return user_image_load(image, names, n_names, UserConstraintKernels{},
+                         UserRiemannianKernels{rmetric_id, nullptr, nullptr, nullptr}, handle);
 }
 
 int mb200_user_target_unload(void* handle) {
@@ -406,12 +441,12 @@ int mb200_leapfrog_euclidean_user(const double* pos_in, const double* mom_in, do
                                   const double* metric_inv, const mb200_model* model,
                                   double* h_out, int32_t* status, int32_t* n_done, void* stream,
                                   const void* user_target) {
-  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  const UserKernels* u;
+  if (const int rc = euclidean_image(user_target, &u)) return rc;
   return leapfrog_euclidean_entry(pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size,
                                   step_sizes, n_steps, n_steps_per_chain, n_flows, coefficients,
                                   initial_h1_flow_step, metric_kind, metric_inv, model, h_out,
-                                  status, n_done, (cudaStream_t)stream, false,
-                                  static_cast<const UserKernels*>(user_target));
+                                  status, n_done, (cudaStream_t)stream, false, u);
 }
 
 int mb200_hamiltonian_euclidean_user(const double* pos, const double* mom, int64_t n_chains,
@@ -433,10 +468,10 @@ int mb200_euclidean_eval_user(const double* pos, const double* mom, int64_t n_ch
                               const mb200_model* model, double* nld_out, double* grad_out,
                               double* vel_out, double* kin_out, void* stream,
                               const void* user_target) {
-  if (!user_target) return fail(MB200_ERR_INVALID_ARG, "user_target is NULL");
+  const UserKernels* u;
+  if (const int rc = euclidean_image(user_target, &u)) return rc;
   return euclidean_eval_impl(pos, mom, n_chains, dim, metric_kind, metric_inv, model, nld_out,
-                             grad_out, vel_out, kin_out, (cudaStream_t)stream,
-                             static_cast<const UserKernels*>(user_target));
+                             grad_out, vel_out, kin_out, (cudaStream_t)stream, u);
 }
 
 int64_t mb200_host_scratch_bytes(int64_t n_chains, int32_t dim) {

@@ -68,22 +68,44 @@ static int rm_launch(Kernel kern, const char* name, RmOp op, int64_t n, int dim,
   return check_launch(name);
 }
 
+// Starts `kern` -- a library kernel, or a kernel of a loaded user image (a cudaKernel_t) -- with
+// the argument types of the library's own instantiations
+template <class... P>
+static void rm_start(void (*kern)(P...), unsigned blocks, int threads, size_t smem,
+                     cudaStream_t st, typename TypeTag<P>::type... args) {
+  void* argv[] = {&args...};
+  cudaLaunchKernel((const void*)kern, dim3(blocks), dim3(threads), argv, smem, st);
+}
+
 // Launch functors of the operations: `run<Target, MetricT>()` starts the operation's kernel for
-// that pair, `global(hadamard)` its global-workspace dense form (api_dense.cu)
+// that pair, `global(hadamard)` its global-workspace dense form (api_dense.cu), `image()` the
+// kernel of the loaded user image `user` (user_riemannian.cuh), planned from the traits the
+// image's policies share with the host (UserRPolicyTraits)
+using ImplicitKernel = decltype(&implicit_leapfrog_kernel<StdGaussianRTarget, QuadraticDiagonalMetric>);
+using VectorKernel = decltype(&riemannian_velocity_kernel<StdGaussianRTarget, QuadraticDiagonalMetric>);
+
 template <RmOp OP>
 struct ImplicitLaunch {
   static constexpr RmOp op = OP;
   const ImplicitArgs& a;
+  const UserRiemannianKernels* user;
   template <class Target, template <class> class MetricT>
   int run() const {
-    auto kern = implicit_leapfrog_kernel<Target, MetricT>;
+    return launch<Target, MetricT>(implicit_leapfrog_kernel<Target, MetricT>);
+  }
+  int image() const {
+    return launch<UserRTargetTraits, UserRPolicyTraits>(
+        reinterpret_cast<ImplicitKernel>(user->implicit));
+  }
+  template <class Target, template <class> class MetricT>
+  int launch(ImplicitKernel kern) const {
     return rm_launch<Target, MetricT>(
         kern, "implicit_leapfrog_kernel", OP, a.n, a.dim, a.m, a.st,
         [&](unsigned blocks, size_t smem, const ModelArgs& margs, int n_mats) {
-          kern<<<blocks, MetricT<Target>::THREADS, smem, a.st>>>(
-              a.q_in, a.p_in, a.q_out, a.p_out, a.dir, a.n, a.dim, a.eps, a.n_steps, margs,
-              a.fp_tol, a.fp_div, a.fp_max, a.rev_tol, a.h_out, a.status, a.n_done, a.fp_iters,
-              n_mats, (int)(OP == RmOp::Midpoint), a.fp_solver);
+          rm_start(kern, blocks, MetricT<Target>::THREADS, smem, a.st, a.q_in, a.p_in, a.q_out,
+                   a.p_out, a.dir, a.n, a.dim, a.eps, a.n_steps, margs, a.fp_tol, a.fp_div,
+                   a.fp_max, a.rev_tol, a.h_out, a.status, a.n_done, a.fp_iters, n_mats,
+                   (int)(OP == RmOp::Midpoint), a.fp_solver);
         });
   }
   int global(bool hadamard) const { return dense_global_implicit(a, hadamard); }
@@ -94,14 +116,22 @@ struct VectorLaunch {
   static constexpr RmOp op = OP;
   static constexpr bool velocity = OP == RmOp::Velocity;
   const VectorArgs& a;
+  const UserRiemannianKernels* user;
   template <class Target, template <class> class MetricT>
   int run() const {
-    auto kern = riemannian_vector_kernel<Target, MetricT, velocity>();
+    return launch<Target, MetricT>(riemannian_vector_kernel<Target, MetricT, velocity>());
+  }
+  int image() const {
+    return launch<UserRTargetTraits, UserRPolicyTraits>(
+        reinterpret_cast<VectorKernel>(velocity ? user->velocity : user->momentum));
+  }
+  template <class Target, template <class> class MetricT>
+  int launch(VectorKernel kern) const {
     return rm_launch<Target, MetricT>(
         kern, velocity ? "riemannian_velocity_kernel" : "riemannian_sample_momentum_kernel", OP,
         a.n, a.dim, a.m, a.st, [&](unsigned blocks, size_t smem, const ModelArgs& margs, int n_mats) {
-          kern<<<blocks, MetricT<Target>::THREADS, smem, a.st>>>(a.q, a.v, a.out, a.n, a.dim,
-                                                                 margs, a.status, n_mats);
+          rm_start(kern, blocks, MetricT<Target>::THREADS, smem, a.st, a.q, a.v, a.out, a.n, a.dim,
+                   margs, a.status, n_mats);
         });
   }
   int global(bool hadamard) const { return dense_global_vector(a, velocity, hadamard); }
@@ -114,8 +144,10 @@ struct WorkspaceQuery {
   int64_t n;
   int dim;
   int64_t* bytes;
+  const UserRiemannianKernels* user = nullptr;
   template <class Target, template <class> class MetricT>
   int run() const { return 0; }
+  int image() const { return 0; }
   int global(bool) const {
     *bytes = dense_global_workspace_bytes(n, dim);
     return 0;
@@ -138,11 +170,20 @@ static int run_on_target(int target_id, const L& l, const char* metric) {
 
 // Which kernel serves a Riemannian model, for every operation L::op: checks the model (the same
 // checks whatever the operation), picks the metric policy and the target, and hands them to `l`.
-// An operation's exclusions sit next to the route they restrict.
+// An operation's exclusions sit next to the route they restrict.  A loaded user image (l.user,
+// the *_user entry points) serves a user target with the image's own user metric.
 template <class L>
 static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
   constexpr RmOp op = L::op;
   const int t = m.target_id;
+  if (l.user != nullptr) {
+    if (t != MB200_TARGET_USER)
+      return fail(MB200_ERR_INVALID_ARG, "user-image entry point needs target_id MB200_TARGET_USER");
+    if (m.rmetric_id != l.user->rmetric_id)
+      return fail(MB200_ERR_INVALID_ARG, "rmetric_id %d does not match the user image's (%d)",
+                  m.rmetric_id, l.user->rmetric_id);
+    return l.image();
+  }
   // one per-chain D x D matrix (the rank-1 metric's Cholesky factor) fits in shared memory
   const bool fits = rm_smem_doubles(dim, 1) * sizeof(double) <= 227 * 1024;
 
@@ -225,24 +266,89 @@ static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
     case MB200_RMETRIC_DIAG_QUADRATIC:
       return run_on_target<QuadraticDiagonalMetric, true>(t, l, "with diagonal / scalar metrics");
     case MB200_RMETRIC_SCALAR_QUADRATIC:
-      return run_on_target<ScalarMetric, true>(t, l, "with diagonal / scalar metrics");
+      return run_on_target<QuadraticScalarMetric, true>(t, l, "with diagonal / scalar metrics");
     default:
       return run_on_target<QuadraticCholeskyMetric, true>(t, l, "with a Cholesky-factored metric");
   }
 }
 
-template <RmOp OP>
-static int implicit_dispatch(const ImplicitArgs& a) {
-  if (a.fp_solver != MB200_FP_SOLVER_DIRECT && a.fp_solver != MB200_FP_SOLVER_STEFFENSEN)
-    return fail(MB200_ERR_INVALID_ARG, "unknown fixed-point solver %d", a.fp_solver);
-  const DeviceScope device_scope(a.q_in);
-  return rm_dispatch(a.m, a.dim, ImplicitLaunch<OP>{a});
+// The handle of a Riemannian *_user entry point: an image of mb200_user_riemannian_load
+static int riemannian_image(const void* handle, const UserRiemannianKernels** u) {
+  if (!handle) return fail(MB200_ERR_INVALID_ARG, "user_image is NULL");
+  *u = &user_riemannian_kernels(handle);
+  if ((*u)->rmetric_id == 0)
+    return fail(MB200_ERR_INVALID_ARG,
+                "user image has no Riemannian kernels (mb200_user_riemannian_load)");
+  return 0;
 }
 
 template <RmOp OP>
-static int vector_dispatch(const VectorArgs& a) {
+static int implicit_dispatch(const ImplicitArgs& a, const UserRiemannianKernels* user = nullptr) {
+  if (a.fp_solver != MB200_FP_SOLVER_DIRECT && a.fp_solver != MB200_FP_SOLVER_STEFFENSEN)
+    return fail(MB200_ERR_INVALID_ARG, "unknown fixed-point solver %d", a.fp_solver);
+  const DeviceScope device_scope(a.q_in);
+  return rm_dispatch(a.m, a.dim, ImplicitLaunch<OP>{a, user});
+}
+
+template <RmOp OP>
+static int vector_dispatch(const VectorArgs& a, const UserRiemannianKernels* user = nullptr) {
   const DeviceScope device_scope(a.q);
-  return rm_dispatch(a.m, a.dim, VectorLaunch<OP>{a});
+  return rm_dispatch(a.m, a.dim, VectorLaunch<OP>{a, user});
+}
+
+// The bodies of the entry points: the registry ones (user == NULL) and their _user twins, whose
+// image serves a user target with its user metric
+
+// implicit leapfrog / midpoint steps (zero steps: the Hamiltonian of the state)
+template <RmOp OP>
+static int implicit_entry(const double* pos_in, const double* mom_in, double* pos_out,
+                          double* mom_out, const int32_t* dir, int64_t n_chains, int dim,
+                          double step_size, const double* step_sizes, int n_steps,
+                          const int32_t* n_steps_per_chain, const mb200_model* model,
+                          int fp_solver, double fp_convergence_tol, double fp_divergence_tol,
+                          int fp_max_iters, double reverse_check_tol, double* h_out,
+                          int32_t* status, int32_t* n_done, int32_t* fp_iters, void* workspace,
+                          int64_t workspace_bytes, void* stream,
+                          const UserRiemannianKernels* user) {
+  if (n_chains == 0 && dim >= 1) return 0;
+  if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
+    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_chains < 0 || dim < 1 || n_steps < 0 || fp_max_iters < 0)
+    return fail(MB200_ERR_INVALID_ARG, "bad sizes");
+  return implicit_dispatch<OP>(
+      ImplicitArgs{pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps,
+                   to_args(model, step_sizes, n_steps_per_chain), fp_convergence_tol,
+                   fp_divergence_tol, fp_max_iters, reverse_check_tol, h_out, status, n_done,
+                   fp_iters, fp_solver, workspace, workspace_bytes, (cudaStream_t)stream},
+      user);
+}
+
+static int hamiltonian_entry(const double* pos, const double* mom, int64_t n_chains, int dim,
+                             const mb200_model* model, double* h_out, int32_t* status,
+                             void* workspace, int64_t workspace_bytes, void* stream,
+                             const UserRiemannianKernels* user) {
+  if (n_chains == 0 && dim >= 1) return 0;
+  if (!pos || !mom || !model || !h_out) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
+  // zero steps: state written back unchanged in place, h evaluated
+  return implicit_dispatch<RmOp::Leapfrog>(
+      ImplicitArgs{pos, mom, const_cast<double*>(pos), const_cast<double*>(mom), nullptr, n_chains,
+                   dim, 0.0, 0, to_args(model), 1e-9, 1e10, 100, 2e-8, h_out, status, nullptr,
+                   nullptr, MB200_FP_SOLVER_DIRECT, workspace, workspace_bytes,
+                   (cudaStream_t)stream},
+      user);
+}
+
+// momentum refresh (SampleMomentum: v = normals) or velocity (Velocity: v = mom)
+template <RmOp OP>
+static int vector_entry(const double* pos, const double* v, double* out, int64_t n_chains,
+                        int dim, const mb200_model* model, int32_t* status, void* stream,
+                        const UserRiemannianKernels* user) {
+  if (n_chains == 0 && dim >= 1) return 0;
+  if (!pos || !v || !out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
+  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
+  return vector_dispatch<OP>(
+      VectorArgs{pos, v, out, n_chains, dim, to_args(model), status, (cudaStream_t)stream}, user);
 }
 
 }  // namespace mb200
@@ -258,17 +364,11 @@ int mb200_implicit_leapfrog_riemannian(
     double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
     double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
     void* workspace, int64_t workspace_bytes, void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
-    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1 || n_steps < 0 || fp_max_iters < 0)
-    return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  if (n_chains == 0) return 0;
-  return implicit_dispatch<RmOp::Leapfrog>(ImplicitArgs{
-      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps,
-      to_args(model, step_sizes, n_steps_per_chain), fp_convergence_tol, fp_divergence_tol,
-      fp_max_iters, reverse_check_tol, h_out, status, n_done, fp_iters, fp_solver, workspace,
-      workspace_bytes, (cudaStream_t)stream});
+  return implicit_entry<RmOp::Leapfrog>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, model, fp_solver, fp_convergence_tol, fp_divergence_tol, fp_max_iters,
+      reverse_check_tol, h_out, status, n_done, fp_iters, workspace, workspace_bytes, stream,
+      nullptr);
 }
 
 // Per-chain buffers live in shared memory except for the global-workspace dense metric policy
@@ -276,6 +376,10 @@ int mb200_implicit_leapfrog_riemannian(
 // library then takes the scratch from the stream-ordered allocator for the duration of the call.
 int64_t mb200_implicit_workspace_bytes(int64_t n_chains, int32_t dim, const mb200_model* model) {
   if (!model || n_chains <= 0 || dim < 1) return 0;
+  // a user image's diagonal / scalar policies keep every per-chain vector in shared memory
+  if (model->rmetric_id == MB200_RMETRIC_USER_DIAGONAL ||
+      model->rmetric_id == MB200_RMETRIC_USER_SCALAR)
+    return 0;
   int64_t bytes = 0;
   rm_dispatch(to_args(model), dim, WorkspaceQuery{n_chains, dim, &bytes});
   return bytes;
@@ -285,15 +389,8 @@ int mb200_hamiltonian_riemannian(const double* pos, const double* mom, int64_t n
                                  int32_t dim, const mb200_model* model, double* h_out,
                                  int32_t* status, void* workspace, int64_t workspace_bytes,
                                  void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos || !mom || !model || !h_out) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  if (n_chains == 0) return 0;
-  // zero steps: state written back unchanged in place, h evaluated
-  return implicit_dispatch<RmOp::Leapfrog>(ImplicitArgs{
-      pos, mom, const_cast<double*>(pos), const_cast<double*>(mom), nullptr, n_chains, dim, 0.0, 0,
-      to_args(model), 1e-9, 1e10, 100, 2e-8, h_out, status, nullptr, nullptr,
-      MB200_FP_SOLVER_DIRECT, workspace, workspace_bytes, (cudaStream_t)stream});
+  return hamiltonian_entry(pos, mom, n_chains, dim, model, h_out, status, workspace,
+                           workspace_bytes, stream, nullptr);
 }
 
 int mb200_selftest_fixed_point(int32_t func_id, int32_t fp_solver, const double* x0,
@@ -339,36 +436,85 @@ int mb200_implicit_midpoint_riemannian(
     double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
     double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
     void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos_in || !mom_in || !pos_out || !mom_out || !model)
-    return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1 || n_steps < 0 || fp_max_iters < 0)
-    return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  return implicit_dispatch<RmOp::Midpoint>(ImplicitArgs{
-      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, n_steps,
-      to_args(model, step_sizes, n_steps_per_chain), fp_convergence_tol, fp_divergence_tol,
-      fp_max_iters, reverse_check_tol, h_out, status, n_done, fp_iters, fp_solver, nullptr, 0,
-      (cudaStream_t)stream});
+  return implicit_entry<RmOp::Midpoint>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, model, fp_solver, fp_convergence_tol, fp_divergence_tol, fp_max_iters,
+      reverse_check_tol, h_out, status, n_done, fp_iters, nullptr, 0, stream, nullptr);
 }
 
 int mb200_sample_momentum_riemannian(const double* pos, const double* normals, double* mom_out,
                                      int64_t n_chains, int32_t dim, const mb200_model* model,
                                      int32_t* status, void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos || !normals || !mom_out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  return vector_dispatch<RmOp::SampleMomentum>(
-      VectorArgs{pos, normals, mom_out, n_chains, dim, to_args(model), status, (cudaStream_t)stream});
+  return vector_entry<RmOp::SampleMomentum>(pos, normals, mom_out, n_chains, dim, model, status,
+                                            stream, nullptr);
 }
 
 int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_out,
                              int64_t n_chains, int32_t dim, const mb200_model* model,
                              int32_t* status, void* stream) {
-  if (n_chains == 0 && dim >= 1) return 0;
-  if (!pos || !mom || !vel_out || !model) return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
-  if (n_chains < 0 || dim < 1) return fail(MB200_ERR_INVALID_ARG, "bad sizes");
-  return vector_dispatch<RmOp::Velocity>(
-      VectorArgs{pos, mom, vel_out, n_chains, dim, to_args(model), status, (cudaStream_t)stream});
+  return vector_entry<RmOp::Velocity>(pos, mom, vel_out, n_chains, dim, model, status, stream,
+                                      nullptr);
+}
+
+// The _user twins: a user target with the user metric of the loaded image `user_image`
+// (mb200_user_riemannian_load), checked first; the registry entry points' bodies otherwise
+
+int mb200_implicit_leapfrog_riemannian_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* workspace, int64_t workspace_bytes, void* stream, const void* user_image) {
+  const UserRiemannianKernels* u;
+  if (const int rc = riemannian_image(user_image, &u)) return rc;
+  return implicit_entry<RmOp::Leapfrog>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, model, fp_solver, fp_convergence_tol, fp_divergence_tol, fp_max_iters,
+      reverse_check_tol, h_out, status, n_done, fp_iters, workspace, workspace_bytes, stream, u);
+}
+
+int mb200_implicit_midpoint_riemannian_user(
+    const double* pos_in, const double* mom_in, double* pos_out, double* mom_out,
+    const int32_t* dir, int64_t n_chains, int32_t dim, double step_size, const double* step_sizes,
+    int32_t n_steps, const int32_t* n_steps_per_chain, const mb200_model* model, int32_t fp_solver,
+    double fp_convergence_tol, double fp_divergence_tol, int32_t fp_max_iters,
+    double reverse_check_tol, double* h_out, int32_t* status, int32_t* n_done, int32_t* fp_iters,
+    void* stream, const void* user_image) {
+  const UserRiemannianKernels* u;
+  if (const int rc = riemannian_image(user_image, &u)) return rc;
+  return implicit_entry<RmOp::Midpoint>(
+      pos_in, mom_in, pos_out, mom_out, dir, n_chains, dim, step_size, step_sizes, n_steps,
+      n_steps_per_chain, model, fp_solver, fp_convergence_tol, fp_divergence_tol, fp_max_iters,
+      reverse_check_tol, h_out, status, n_done, fp_iters, nullptr, 0, stream, u);
+}
+
+int mb200_hamiltonian_riemannian_user(const double* pos, const double* mom, int64_t n_chains,
+                                      int32_t dim, const mb200_model* model, double* h_out,
+                                      int32_t* status, void* workspace, int64_t workspace_bytes,
+                                      void* stream, const void* user_image) {
+  const UserRiemannianKernels* u;
+  if (const int rc = riemannian_image(user_image, &u)) return rc;
+  return hamiltonian_entry(pos, mom, n_chains, dim, model, h_out, status, workspace,
+                           workspace_bytes, stream, u);
+}
+
+int mb200_sample_momentum_riemannian_user(const double* pos, const double* normals,
+                                          double* mom_out, int64_t n_chains, int32_t dim,
+                                          const mb200_model* model, int32_t* status, void* stream,
+                                          const void* user_image) {
+  const UserRiemannianKernels* u;
+  if (const int rc = riemannian_image(user_image, &u)) return rc;
+  return vector_entry<RmOp::SampleMomentum>(pos, normals, mom_out, n_chains, dim, model, status,
+                                            stream, u);
+}
+
+int mb200_dh_dmom_riemannian_user(const double* pos, const double* mom, double* vel_out,
+                                  int64_t n_chains, int32_t dim, const mb200_model* model,
+                                  int32_t* status, void* stream, const void* user_image) {
+  const UserRiemannianKernels* u;
+  if (const int rc = riemannian_image(user_image, &u)) return rc;
+  return vector_entry<RmOp::Velocity>(pos, mom, vel_out, n_chains, dim, model, status, stream, u);
 }
 
 }  // extern "C"

@@ -19,7 +19,11 @@
 // grad_quadratic_form_inv (matrices.py:1679-1685) need, and because it parallelises over a CTA
 // without any serial tridiagonal phase.
 #pragma once
+#ifndef __CUDACC_RTC__
 #include <cfloat>
+#elif !defined(DBL_EPSILON)
+#define DBL_EPSILON 2.2204460492503131e-16  // NVRTC (user_riemannian.cuh) has no <cfloat>
+#endif
 
 #include "common.cuh"
 
@@ -860,6 +864,7 @@ __device__ inline void smem_matmul(const Blk& k, int n, int ld, const double* X,
   __syncthreads();
 }
 
+#ifndef __CUDACC_RTC__  // library self-tests: kept out of the run-time compiled user images
 // Diagnostic kernel: K3 on arbitrary dense symmetric matrices (one CTA per matrix).  With
 // `warm_from` >= 0 the solve of matrix i is warm-started from the eigenvectors of matrix
 // `warm_from` (exercising the V^T H V path used between fixed-point iterates).
@@ -910,6 +915,7 @@ static __global__ void __launch_bounds__(RM_THREADS)
     if (blk.tid == 0) status[mi] = ok ? 0 : MB200_STATUS_LINALG;
   }
 }
+#endif
 
 // ---------------------------------------------------------------------------------------------
 // K2: in-place lower Cholesky factor of the SPD matrix M [dim x dim, stride ld]
@@ -1488,9 +1494,23 @@ using QuadraticDiagonalMetric = DiagonalMetric<Target, QuadraticDiagModel>;
 template <class Target>
 using FunnelFisherMetric = DiagonalMetric<Target, FunnelFisherDiagModel>;
 
-// MB200_RMETRIC_SCALAR_QUADRATIC: M(q) = s(q) I with s = a + b |q|^2, vjp(w) = 2 b w q.  The
-// scalar and its reciprocal are block-uniform registers.
-template <class Target>
+// scalar models s(q) and their VJPs w -> w ds/dq (w a block-uniform scalar), over dim entries
+// MB200_RMETRIC_SCALAR_QUADRATIC: s = a + b |q|^2, vjp(w)_i = 2 b w q_i
+struct QuadraticScalarModel {
+  double a, b;
+  __device__ QuadraticScalarModel(const ModelArgs& m, int) : a(m.mp[0]), b(m.mp[1]) {}
+  __device__ double scalar(const Blk& k, int dim, const double* q) const {
+    double acc = 0.0;
+    for (int i = k.tid; i < dim; i += k.nthr) acc = fma(q[i], q[i], acc);
+    return a + b * block_sum(k, acc);
+  }
+  __device__ void vjp(const Blk& k, int dim, const double* q, double g, double* out) const {
+    for (int i = k.tid; i < dim; i += k.nthr) out[i] = 2.0 * b * g * q[i];
+  }
+};
+
+// M(q) = s(q) I.  The scalar and its reciprocal are block-uniform registers.
+template <class Target, class Model>
 struct ScalarMetric {
   static constexpr bool SOFTABS = false;
   static constexpr bool COMPACT = true;
@@ -1498,16 +1518,15 @@ struct ScalarMetric {
   static constexpr int MIN_BLOCKS = RM_COMPACT_MIN_BLOCKS;
   static constexpr int THREADS = RM_COMPACT_THREADS;
   const Target& t;
-  double a, b, s, inv_s;
+  Model model;
+  double s, inv_s;
   __device__ ScalarMetric(const Target& tt, const ModelArgs& m)
-      : t(tt), a(m.mp[0]), b(m.mp[1]), s(1.0), inv_s(1.0) {}
+      : t(tt), model(m, tt.dim), s(1.0), inv_s(1.0) {}
   __device__ void reset() {}
 
   // LinAlgError status unless s > 0 (NaN fails): PositiveScaledIdentityMatrix (matrices.py:692-694)
   __device__ int build(const Blk& k, RmWork& w, const double* q) {
-    double acc = 0.0;
-    for (int i = k.tid; i < w.dim; i += k.nthr) acc = fma(q[i], q[i], acc);
-    s = a + b * block_sum(k, acc);
+    s = model.scalar(k, w.dim, q);
     inv_s = 1.0 / s;
     return (s > 0.0) ? 0 : MB200_STATUS_LINALG;
   }
@@ -1528,7 +1547,7 @@ struct ScalarMetric {
   // vjp(D / s)  (grad_log_abs_det, matrices.py:669-670)
   __device__ void vjp_grad_log_abs_det(const Blk& k, RmWork& w, const double* q, double* out) {
     const double g = w.dim / s;
-    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = 2.0 * b * g * q[i];
+    model.vjp(k, w.dim, q, g, out);
     __syncthreads();
   }
   // vjp(-sum(p ** 2) / s ** 2)  (grad_quadratic_form_inv, matrices.py:672-673)
@@ -1537,9 +1556,27 @@ struct ScalarMetric {
     double acc = 0.0;
     for (int i = k.tid; i < w.dim; i += k.nthr) acc = fma(p[i], p[i], acc);
     const double g = -block_sum(k, acc) / (s * s);
-    for (int i = k.tid; i < w.dim; i += k.nthr) out[i] = 2.0 * b * g * q[i];
+    model.vjp(k, w.dim, q, g, out);
     __syncthreads();
   }
+};
+
+template <class Target>
+using QuadraticScalarMetric = ScalarMetric<Target, QuadraticScalarModel>;
+
+// What the host's launch plan (rm_launch) reads of a user image's policies, DiagonalMetric and
+// ScalarMetric over the user functions of user_riemannian.cuh: that header, which NVRTC compiles,
+// checks that its policies carry these values.
+struct UserRTargetTraits {
+  static constexpr bool DENSE_MTP = false;
+};
+template <class>
+struct UserRPolicyTraits {
+  static constexpr bool SOFTABS = false;
+  static constexpr bool COMPACT = true;
+  static constexpr int N_MATS = 0;
+  static constexpr int MIN_BLOCKS = RM_COMPACT_MIN_BLOCKS;
+  static constexpr int THREADS = RM_COMPACT_THREADS;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -1759,6 +1796,7 @@ __device__ inline int fixed_point_steffensen(const Blk& k, int dim, double* xa, 
   return MB200_STATUS_CONVERGENCE;
 }
 
+#ifndef __CUDACC_RTC__  // library self-tests: kept out of the run-time compiled user images
 // Diagnostic kernel: K4 on the reference's own known-answer problems
 // (reference tests/test_solvers.py:25-47): 0 babylonian (y/x + x)/2, 1 ratio (x+y)/(x+1),
 // 2 cosine, 3 doubling 2x, 4 quadratic 1 + x^2.  One CTA per problem instance.
@@ -1806,6 +1844,7 @@ static __global__ void __launch_bounds__(64)
     }
   }
 }
+#endif
 
 // ---------------------------------------------------------------------------------------------
 // K4 + K5: the integrator

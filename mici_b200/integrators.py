@@ -483,7 +483,7 @@ class _ImplicitIntegrator(Integrator):
             self.fixed_point_solver.kind, float(kw["convergence_tol"]),
             float(kw["divergence_tol"]), int(kw["max_iters"]), float(self.reverse_check_tol),
             _lib.ptr(h), _lib.ptr(status), _lib.ptr(n_done), _lib.ptr(iters), *ws_args,
-            _lib.current_stream_ptr(dev))
+            _lib.current_stream_ptr(dev), target=sysm._user_pair)
         return iters
 
 

@@ -14,6 +14,11 @@ A constrained user target (``n_constr >= 1``, contract: ``csrc/user_constraint.c
 carries the constrained leapfrog and projection kernels (``csrc/constrained.cuh``) for its
 constraint count and KP; its cache key covers both and whether the source defines
 ``mhp_constr``.
+
+A user target paired with a user diagonal or scalar metric (contract:
+``csrc/user_riemannian.cuh``) compiles into an image of its own: the implicit-integrator, velocity
+and momentum-refresh kernels of ``csrc/riemannian.cuh`` for that (target, metric) pair, keyed on
+both sources and the metric kind.
 """
 
 from __future__ import annotations
@@ -25,6 +30,7 @@ import os
 import threading
 
 from .errors import Error, TargetCompileError
+from .targets import RMETRIC_USER_DIAGONAL, RMETRIC_USER_SCALAR
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_PKG, "csrc")
@@ -52,6 +58,20 @@ def constrained_name_expressions(kp):
                  for k in ("leapfrog", "project") for g in ("false", "true"))
 
 
+# The kernels of a Riemannian image, in the kernel-table order of mb200_user_riemannian_load:
+# implicit leapfrog / midpoint, velocity, momentum refresh
+RIEMANNIAN_KINDS = ("diagonal", "scalar")
+# the rmetric_id a Riemannian image serves, by metric kind
+RIEMANNIAN_RMETRIC_IDS = {"diagonal": RMETRIC_USER_DIAGONAL, "scalar": RMETRIC_USER_SCALAR}
+
+
+def riemannian_name_expressions(kind):
+    m = "mb200::User%sMetric" % kind.capitalize()
+    return tuple(f"&mb200::{k}<mb200::UserRTarget, {m}>"
+                 for k in ("implicit_leapfrog_kernel", "riemannian_velocity_kernel",
+                           "riemannian_sample_momentum_kernel"))
+
+
 def constrained_kp(dim, n_constr):
     """KP (coordinates per lane / 2) of the constrained kernel for ``dim``, chosen as for the
     registry's sphere and multi-sphere targets; ``None`` outside dim <= 256 (one constraint) or
@@ -64,9 +84,10 @@ _lock = threading.Lock()
 _nvrtc = None
 _images = {}   # key -> (cubin bytes, lowered names)
 _handles = {}  # key -> loaded library handle (ctypes.c_void_p)
-# (source, name, constraint) -> key / handle: a repeat lookup, once per launch of a user target,
-# is one dict access; the headers are hashed and NVRTC's version read once per process
+# (source, name, constraint, metric) -> key / handle: a repeat lookup, once per launch of a user
+# target, is one dict access; the headers are hashed and NVRTC's version read once per process
 # (_static_key).  constraint: () for an unconstrained target, else (n_constr, kp, mhp_constr).
+# metric: () for a Euclidean image, else (kind, metric source, metric name) of a Riemannian one.
 _keys = {}
 _loaded = {}
 _static = None
@@ -158,9 +179,16 @@ def _headers_digest():
     return h.hexdigest()
 
 
-def translation_unit(source, name="user_target", constraint=()):
+def translation_unit(source, name="user_target", constraint=(), metric=()):
     """The program NVRTC compiles: the engine header, then the user source with its own line
-    numbers (``#line``), so that compile errors point at the user's lines."""
+    numbers (``#line``), so that compile errors point at the user's lines.  A Riemannian image
+    adds the metric source, then binds the metric functions on the line after its last one."""
+    if metric:
+        _, msource, mname = metric
+        end = len(msource.splitlines()) + 1
+        return (f'#include "user_riemannian.cuh"\n#line 1 "{name}.cu"\n{source}\n'
+                f'#line 1 "{mname}.cu"\n{msource}\n#line {end} "{mname}.cu"\n'
+                "MB200_USER_METRIC_FUNCTIONS\n")
     header = "user_constraint.cuh" if constraint else "user_target.cuh"
     return f'#include "{header}"\n#line 1 "{name}.cu"\n{source}\n'
 
@@ -173,14 +201,27 @@ def _constraint(n_constr, kp, mhp_constr):
     return (int(n_constr), int(kp), bool(mhp_constr))
 
 
-def _defines(constraint):
+def _metric(metric):
+    if not metric:
+        return ()
+    kind, msource, mname = metric
+    if kind not in RIEMANNIAN_KINDS:
+        raise ValueError(f"bad Riemannian image: metric kind {kind!r}")
+    return (kind, str(msource), str(mname))
+
+
+def _defines(constraint, metric=()):
+    if metric:
+        return ("-DMB200_USER_%s_METRIC" % metric[0].upper(),)
     if not constraint:
         return ()
     n_constr, _, mhp = constraint
     return (f"-DMB200_USER_N_CONSTR={n_constr}",) + (("-DMB200_USER_MHP_CONSTR",) if mhp else ())
 
 
-def _name_expressions(constraint):
+def _name_expressions(constraint, metric=()):
+    if metric:
+        return riemannian_name_expressions(metric[0])
     return NAME_EXPRESSIONS + (constrained_name_expressions(constraint[1]) if constraint else ())
 
 
@@ -193,49 +234,55 @@ def _static_key():
     return _static
 
 
-def cache_key(source, name="user_target", constraint=()):
+def cache_key(source, name="user_target", constraint=(), metric=()):
     parts = [_static_key(), name, source]
     if constraint:
         parts.append("n_constr=%d kp=%d mhp_constr=%d" % constraint)
+    if metric:
+        parts += ["riemannian metric=" + metric[0], metric[2], metric[1]]
     return hashlib.sha256("\0".join(parts).encode()).hexdigest()
 
 
-def compile_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=False):
+def compile_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=False,
+                   metric=None):
     """Compile a user target; returns ``(key, cubin, lowered kernel names)``, from the process
     cache when the same source was compiled before.  ``n_constr >= 1``: a constrained target,
-    whose image also carries the constrained kernels at ``kp``.  Raises ``TargetCompileError``
-    with the NVRTC log on failure."""
+    whose image also carries the constrained kernels at ``kp``.  ``metric = (kind, source,
+    name)``, kind ``"diagonal"`` or ``"scalar"``: the Riemannian image of the target with that
+    user metric.  Raises ``TargetCompileError`` with the NVRTC log on failure."""
     constraint = _constraint(n_constr, kp, mhp_constr)
+    metric = _metric(metric)
+    lookup = (source, name, constraint, metric)
     with _lock:
-        key = _keys.get((source, name, constraint))
+        key = _keys.get(lookup)
         if key is not None:
             stats["hits"] += 1
             return key, *_images[key]
-    key = cache_key(source, name, constraint)
+    key = cache_key(source, name, constraint, metric)
     with _lock:
         if key in _images:  # the same program under another (source, name) spelling
             stats["hits"] += 1
-            _keys[(source, name, constraint)] = key
+            _keys[lookup] = key
             return key, *_images[key]
-    cubin, names = _compile(source, name, constraint)
+    cubin, names = _compile(source, name, constraint, **({"metric": metric} if metric else {}))
     with _lock:
         _images.setdefault(key, (cubin, names))
-        _keys[(source, name, constraint)] = key
+        _keys[lookup] = key
         stats["compiles"] += 1
         return key, *_images[key]
 
 
-def _compile(source, name, constraint=()):
+def _compile(source, name, constraint=(), metric=()):
     lib = nvrtc()
     prog = ctypes.c_void_p()
-    src = translation_unit(source, name, constraint).encode()
-    exprs = _name_expressions(constraint)
+    src = translation_unit(source, name, constraint, metric).encode()
+    exprs = _name_expressions(constraint, metric)
     _ok(lib.nvrtcCreateProgram(ctypes.byref(prog), src, f"{name}_tu.cu".encode(), 0, None, None),
         "nvrtcCreateProgram")
     try:
         for expr in exprs:
             _ok(lib.nvrtcAddNameExpression(prog, expr.encode()), "nvrtcAddNameExpression")
-        opts = [o.encode() for o in OPTIONS + _defines(constraint)] + [
+        opts = [o.encode() for o in OPTIONS + _defines(constraint, metric)] + [
             f"-I{CSRC}".encode(), f"-I{INCLUDE}".encode()]
         argv = (ctypes.c_char_p * len(opts))(*opts)
         rc = lib.nvrtcCompileProgram(prog, len(opts), ctypes.cast(argv, ctypes.c_void_p))
@@ -263,30 +310,35 @@ def _compile(source, name, constraint=()):
         lib.nvrtcDestroyProgram(ctypes.byref(prog))
 
 
-def load_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=False):
-    """Handle of the loaded image of a user target (``mb200_user_target_load``, or
-    ``mb200_user_constraint_load`` for a constrained one), compiled and loaded once per
-    process."""
+def load_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=False, metric=None):
+    """Handle of the loaded image of a user target (``mb200_user_target_load``,
+    ``mb200_user_constraint_load`` for a constrained one, ``mb200_user_riemannian_load`` with a
+    user metric), compiled and loaded once per process."""
     from . import _lib  # noqa: PLC0415
 
     constraint = _constraint(n_constr, kp, mhp_constr)
+    metric = _metric(metric)
+    lookup = (source, name, constraint, metric)
     with _lock:
-        handle = _loaded.get((source, name, constraint))
+        handle = _loaded.get(lookup)
     if handle is not None:
         return handle
     key, cubin, names = compile_target(source, name, n_constr=n_constr, kp=kp,
-                                       mhp_constr=mhp_constr)
+                                       mhp_constr=mhp_constr, metric=metric)
     with _lock:
         handle = _handles.get(key)
         if handle is None:
             arr = (ctypes.c_char_p * len(names))(*[n.encode() for n in names])
             handle = ctypes.c_void_p()
-            if constraint:
+            if metric:
+                _lib.call("mb200_user_riemannian_load", cubin, len(cubin), arr, len(names),
+                          RIEMANNIAN_RMETRIC_IDS[metric[0]], ctypes.byref(handle))
+            elif constraint:
                 _lib.call("mb200_user_constraint_load", cubin, len(cubin), arr, len(names),
                           *constraint, ctypes.byref(handle))
             else:
                 _lib.call("mb200_user_target_load", cubin, len(cubin), arr, len(names),
                           ctypes.byref(handle))
             _handles[key] = handle
-        _loaded[(source, name, constraint)] = handle
+        _loaded[lookup] = handle
     return handle

@@ -30,6 +30,9 @@ from .errors import LinAlgError
 from .solvers import solve_projection_onto_manifold_newton
 from .targets import (
     RMETRIC_SOFTABS,
+    CudaDiagonalMetric,
+    CudaRiemannianPair,
+    CudaScalarMetric,
     CudaTarget,
     FunnelFisherMetric,
     HadamardMetric,
@@ -187,7 +190,8 @@ def _dir_tensor(d, n, device):
 class System:
     """Base class (systems.py:39-229): holds the target model and builds ``mb200_model``."""
 
-    # whether a user-written `CudaTarget` may drive the system (its kernels need only l and grad l)
+    # whether a user-written `CudaTarget` may drive the system (its kernels need only l and grad l);
+    # a Riemannian system sets it on the instance when it is given a user metric
     _user_targets = False
 
     def __init__(self, neg_log_dens, *, grad_neg_log_dens=None, backend=None):
@@ -198,7 +202,7 @@ class System:
                 "not supported."
             )
             raise TypeError(msg)
-        if isinstance(neg_log_dens, CudaTarget) and not type(self)._user_targets:
+        if isinstance(neg_log_dens, CudaTarget) and not self._user_targets:
             raise TypeError(f"{type(self).__name__} does not take a CudaTarget: user targets run "
                             "on EuclideanMetricSystem.")
         if grad_neg_log_dens is not None or backend is not None:
@@ -647,6 +651,20 @@ class GaussianDenseConstrainedEuclideanMetricSystem(GaussianEuclideanMetricSyste
 class RiemannianMetricSystem(System):
     """Riemannian Hamiltonian system with a position-dependent metric (systems.py:1187-1402)."""
 
+    # the (CudaTarget, user metric) pair whose image the launches run, None for registry models
+    _user_pair = None
+
+    def _accept_user_metric(self, target, metric, cls):
+        """Before ``System.__init__``: a user metric of class ``cls`` comes with an unconstrained
+        ``CudaTarget``, which the system then takes."""
+        if not isinstance(metric, cls):
+            return
+        if not isinstance(target, CudaTarget) or target.n_constr:
+            raise TypeError(f"A {cls.__name__} needs an unconstrained CudaTarget as "
+                            "`neg_log_dens`.")
+        self._user_targets = True
+        self._user_pair = CudaRiemannianPair(target, metric)
+
     def _workspace(self, n, dim, device):
         model = self._model(device)
         nbytes = int(_lib.load().mb200_implicit_workspace_bytes(n, dim, ctypes.byref(model)))
@@ -664,7 +682,7 @@ class RiemannianMetricSystem(System):
             model = self._model(dev)
             _lib.call("mb200_hamiltonian_riemannian", _lib.ptr(pos), _lib.ptr(mom), n, dim,
                       ctypes.byref(model), _lib.ptr(h), _lib.ptr(status), _lib.ptr(ws),
-                      ws.numel(), _lib.current_stream_ptr(dev))
+                      ws.numel(), _lib.current_stream_ptr(dev), target=self._user_pair)
             return h
 
         return _on_batch(state, launch)
@@ -679,7 +697,8 @@ class RiemannianMetricSystem(System):
             status = torch.empty(n, dtype=torch.int32, device=dev)
             model = self._model(dev)
             _lib.call("mb200_dh_dmom_riemannian", _lib.ptr(pos), _lib.ptr(mom), _lib.ptr(vel), n,
-                      dim, ctypes.byref(model), _lib.ptr(status), _lib.current_stream_ptr(dev))
+                      dim, ctypes.byref(model), _lib.ptr(status), _lib.current_stream_ptr(dev),
+                      target=self._user_pair)
             _check_metric_status(status, n)
             return vel
 
@@ -703,7 +722,8 @@ class RiemannianMetricSystem(System):
         status = torch.empty(n, dtype=torch.int32, device=dev)
         model = self._model(dev)
         _lib.call("mb200_sample_momentum_riemannian", _lib.ptr(pos), _lib.ptr(z), _lib.ptr(out),
-                  n, dim, ctypes.byref(model), _lib.ptr(status), _lib.current_stream_ptr(dev))
+                  n, dim, ctypes.byref(model), _lib.ptr(status), _lib.current_stream_ptr(dev),
+                  target=self._user_pair)
         _check_metric_status(status, n)
         return _like_input(state.pos, out[0] if single else out)
 
@@ -749,7 +769,8 @@ class SoftAbsRiemannianMetricSystem(RiemannianMetricSystem):
 class ScalarRiemannianMetricSystem(RiemannianMetricSystem):
     """Scaled-identity position-dependent metric ``s(q) I`` (systems.py:1405-1490) with
     ``PositiveScaledIdentityMatrix`` arithmetic (matrices.py:595-706): ``metric_scalar_func`` is a
-    registered metric model, ``mici_b200.targets.QuadraticScalarMetric`` (s = a + b |q|^2).
+    registered metric model, ``mici_b200.targets.QuadraticScalarMetric`` (s = a + b |q|^2), or a
+    user-written ``mici_b200.targets.CudaScalarMetric`` with a ``CudaTarget``.
 
     A chain whose ``s(q)`` is not positive fails with status 3 (``LinAlgError``) outside a
     fixed-point solve and with ``ConvergenceError`` inside one; the reference raises
@@ -757,15 +778,17 @@ class ScalarRiemannianMetricSystem(RiemannianMetricSystem):
 
     def __init__(self, neg_log_dens, metric_scalar_func, *, vjp_metric_scalar_func=None,
                  grad_neg_log_dens=None, backend=None):
+        self._accept_user_metric(neg_log_dens, metric_scalar_func, CudaScalarMetric)
         super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
-        if not isinstance(metric_scalar_func, QuadraticScalarMetric):
+        if not isinstance(metric_scalar_func, (QuadraticScalarMetric, CudaScalarMetric)):
             raise TypeError("`metric_scalar_func` must be a registered metric model "
-                            "(QuadraticScalarMetric).")
+                            "(QuadraticScalarMetric) or a CudaScalarMetric.")
         if vjp_metric_scalar_func is not None:
             raise ValueError("The metric VJP is fused into the kernels.")
         self.metric_model = metric_scalar_func
         self._rmetric_id = metric_scalar_func.rmetric_id
         self._rmetric_params = metric_scalar_func.params
+        self._rmetric_aux = metric_scalar_func.aux
 
 
 class DiagonalRiemannianMetricSystem(RiemannianMetricSystem):
@@ -773,7 +796,8 @@ class DiagonalRiemannianMetricSystem(RiemannianMetricSystem):
     ``PositiveDiagonalMatrix`` arithmetic (matrices.py:709-792): ``metric_diagonal_func`` is a
     registered metric model -- ``mici_b200.targets.QuadraticDiagonalMetric`` (d_i = a + b q_i^2)
     or ``mici_b200.targets.FunnelFisherMetric`` (the funnel's expected Fisher information, funnel
-    target only).  O(D) per metric: a chain's whole state lives in a small CTA's shared memory.
+    target only) -- or a user-written ``mici_b200.targets.CudaDiagonalMetric`` with a
+    ``CudaTarget``.  O(D) per metric: a chain's whole state lives in a small CTA's shared memory.
 
     A chain whose ``d(q)`` has an entry that is not positive fails with status 3
     (``LinAlgError``) outside a fixed-point solve and with ``ConvergenceError`` inside one; the
@@ -781,10 +805,13 @@ class DiagonalRiemannianMetricSystem(RiemannianMetricSystem):
 
     def __init__(self, neg_log_dens, metric_diagonal_func, *, vjp_metric_diagonal_func=None,
                  grad_neg_log_dens=None, backend=None):
+        self._accept_user_metric(neg_log_dens, metric_diagonal_func, CudaDiagonalMetric)
         super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
-        if not isinstance(metric_diagonal_func, (QuadraticDiagonalMetric, FunnelFisherMetric)):
+        if not isinstance(metric_diagonal_func,
+                          (QuadraticDiagonalMetric, FunnelFisherMetric, CudaDiagonalMetric)):
             raise TypeError("`metric_diagonal_func` must be a registered metric model "
-                            "(QuadraticDiagonalMetric or FunnelFisherMetric).")
+                            "(QuadraticDiagonalMetric or FunnelFisherMetric) or a "
+                            "CudaDiagonalMetric.")
         if isinstance(metric_diagonal_func, FunnelFisherMetric) and not isinstance(
                 neg_log_dens, NealFunnel):
             raise TypeError("FunnelFisherMetric is the metric of the NealFunnel target.")
@@ -793,6 +820,7 @@ class DiagonalRiemannianMetricSystem(RiemannianMetricSystem):
         self.metric_model = metric_diagonal_func
         self._rmetric_id = metric_diagonal_func.rmetric_id
         self._rmetric_params = metric_diagonal_func.params
+        self._rmetric_aux = metric_diagonal_func.aux
 
 
 class CholeskyFactoredRiemannianMetricSystem(RiemannianMetricSystem):

@@ -29,6 +29,8 @@ RMETRIC_DIAG_QUADRATIC = 3
 RMETRIC_DIAG_FUNNEL_FISHER = 4
 RMETRIC_SCALAR_QUADRATIC = 5
 RMETRIC_CHOL_QUADRATIC = 6
+RMETRIC_USER_DIAGONAL = 32  # MB200_RMETRIC_USER_DIAGONAL: CudaDiagonalMetric
+RMETRIC_USER_SCALAR = 33  # MB200_RMETRIC_USER_SCALAR: CudaScalarMetric
 
 
 class Target:
@@ -234,9 +236,94 @@ class CudaTarget(Target):
         return f"CudaTarget(dim={self.dim}, name={self.name!r}, params={self.params}{extra})"
 
 
+class _CudaMetric:
+    """A user-written diagonal or scalar metric (contract: ``mici_b200/csrc/user_riemannian.cuh``):
+    CUDA C++ source, at most 8 ``params`` (``c.params`` inside the metric functions) and an
+    optional ``aux`` array (``c.aux``).  It runs with a ``CudaTarget`` only, compiled with it into
+    one image; like the target it holds only source, params and aux."""
+
+    kind = ""
+    rmetric_id = -1
+
+    def __init__(self, source, params=(), aux=None, name=None):
+        if not isinstance(source, str):
+            raise ValueError("`source` must be a string of CUDA C++.")
+        try:
+            params = tuple(float(x) for x in params)
+        except (TypeError, ValueError) as e:
+            raise ValueError(f"`params` must be an iterable of scalars: {e}") from e
+        if len(params) > 8:
+            raise ValueError(f"{type(self).__name__} takes at most 8 params, got {len(params)}.")
+        if aux is not None:
+            try:
+                aux = np.ascontiguousarray(aux, dtype=np.float64)
+            except (TypeError, ValueError) as e:
+                raise ValueError(f"`aux` cannot be converted to a float64 array: {e}") from e
+        self.source = source
+        self.params = params
+        self.aux = aux
+        self.name = "user_metric" if name is None else str(name)
+        if not self.name.isidentifier():
+            raise ValueError("`name` must be a valid identifier.")
+
+    def __repr__(self):
+        return f"{type(self).__name__}(name={self.name!r}, params={self.params})"
+
+
+class CudaDiagonalMetric(_CudaMetric):
+    """A user-written diagonal metric M(q) = diag(d(q)) for ``DiagonalRiemannianMetricSystem``:
+    CUDA C++ source defining
+
+        __device__ void metric_diagonal(const mb200::Chain& c, double* d);
+        __device__ void vjp_metric_diagonal(const mb200::Chain& c, const double* w, double* out);
+
+    with ``out[j] = sum_i w[i] dd_i/dq_j``."""
+
+    kind = "diagonal"
+    rmetric_id = RMETRIC_USER_DIAGONAL
+
+
+class CudaScalarMetric(_CudaMetric):
+    """A user-written scalar metric M(q) = s(q) I for ``ScalarRiemannianMetricSystem``: CUDA C++
+    source defining
+
+        __device__ double metric_scalar(const mb200::Chain& c);
+        __device__ void vjp_metric_scalar(const mb200::Chain& c, double w, double* out);
+
+    with ``out[j] = w ds/dq_j``."""
+
+    kind = "scalar"
+    rmetric_id = RMETRIC_USER_SCALAR
+
+
+class CudaRiemannianPair:
+    """A ``CudaTarget`` with a user metric: what a Riemannian system with a user metric runs,
+    compiled into one image (``mb200_user_riemannian_load``)."""
+
+    def __init__(self, target, metric):
+        self.target, self.metric = target, metric
+
+    def _metric_key(self):
+        return (self.metric.kind, self.metric.source, self.metric.name)
+
+    def compile(self):
+        """Compile now (raises ``mici_b200.errors.TargetCompileError``); returns ``self``."""
+        from . import jit  # noqa: PLC0415
+
+        jit.compile_target(self.target.source, self.target.name, metric=self._metric_key())
+        return self
+
+    def handle(self):
+        """The loaded device image of this pair, from the process cache."""
+        from . import jit  # noqa: PLC0415
+
+        return jit.load_target(self.target.source, self.target.name, metric=self._metric_key())
+
+
 def user_handle(target):
-    """The loaded image of a ``CudaTarget``, or ``None`` for a registry target."""
-    return target.handle() if isinstance(target, CudaTarget) else None
+    """The loaded image of a ``CudaTarget`` or of a ``CudaRiemannianPair``, or ``None`` for a
+    registry target."""
+    return target.handle() if isinstance(target, (CudaTarget, CudaRiemannianPair)) else None
 
 
 class Rank1Metric:
