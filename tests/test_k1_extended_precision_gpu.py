@@ -26,18 +26,13 @@ import torch
 from mici_b200 import _lib, problems, systems
 from mici_b200 import targets as mtargets
 from oracle import mici_oracle as mo
-from oracle import targets as otargets
+
+from extended_precision import (BANANA_B, ULP, L, _check_ratio, _GivenInverse, _h_terms,
+                                _oracle_target, _rel_err, leapfrog_ext, need_extended)
 
 DEV = "cuda:0"
-L = np.longdouble
-ULP = 2.0**-52  # float64 epsilon: errors below are reported in these units
-EXTENDED = np.finfo(np.longdouble).nmant >= 63
-need_extended = pytest.mark.skipif(
-    not EXTENDED, reason=f"np.longdouble has a {np.finfo(np.longdouble).nmant}-bit mantissa, "
-    "the extended-precision reference needs >= 63")
 
 TARGETS = ["std_gaussian", "neal_funnel", "banana"]
-BANANA_B = 0.5
 STEP = {"std_gaussian": 0.1, "neal_funnel": 0.01, "banana": 0.05}
 # dimensions on both sides of each class boundary of the kernel's padded width DP (even only for
 # the banana, whose coordinates come in pairs)
@@ -95,86 +90,6 @@ def _batch(layout, sms):
 def _mts(n, sms):
     """Set of group tile counts (MT) that occur in a batch of n chains."""
     return {mt for _, t in _passes(n, sms) for mt in _group_tiles(t) if mt > 0}
-
-
-# ------------------------------------------------------------------------------------------------
-# Extended-precision reference (formulas of oracle/targets.py, schedule of
-# mici_oracle.leapfrog_steps: half kick, drift with M^-1, half kick with the memoised gradient,
-# the two half kicks at a step boundary applied separately)
-# ------------------------------------------------------------------------------------------------
-
-
-def _grad(target, q):
-    dim = q.shape[1]
-    if target == "std_gaussian":
-        return q.copy()
-    g = np.empty_like(q)
-    if target == "neal_funnel":
-        v, x = q[:, :1], q[:, 1:]
-        e = np.exp(-v)
-        g[:, :1] = v / L(9) + L(0.5) * (dim - 1) - L(0.5) * e * (x * x).sum(1, keepdims=True)
-        g[:, 1:] = e * x
-        return g
-    b = L(BANANA_B)
-    x, y = q[:, 0::2], q[:, 1::2]
-    r = y - b * x * x
-    g[:, 0::2] = x / L(4) - L(2) * b * x * r
-    g[:, 1::2] = r
-    return g
-
-
-def _h_terms(target, q, p, a):
-    """Per-chain h(q, p) = l(q) + p . M^-1 p / 2 and the sum of the absolute values of its terms
-    (the scale its rounding error is measured against: the funnel's l cancels)."""
-    dim = q.shape[1]
-    kin = L(0.5) * np.einsum("ij,ij->i", p, p @ a.T)
-    if target == "std_gaussian":
-        terms = [L(0.5) * (q * q).sum(1)]
-    elif target == "neal_funnel":
-        v, x = q[:, 0], q[:, 1:]
-        terms = [v * v / L(18), L(0.5) * (dim - 1) * v, L(0.5) * np.exp(-v) * (x * x).sum(1)]
-    else:
-        b = L(BANANA_B)
-        x, y = q[:, 0::2], q[:, 1::2]
-        r = y - b * x * x
-        terms = [(x * x / L(8)).sum(1), (L(0.5) * r * r).sum(1)]
-    h = sum(terms) + kin
-    scale = sum(np.abs(t) for t in terms) + np.abs(kin)
-    return h, scale
-
-
-def leapfrog_ext(target, q, p, time_step, n_steps, minv):
-    """n_steps leapfrog steps of every row of (q, p) in long double; time_step[c] = dir * eps_c."""
-    q, p, a = q.astype(L), p.astype(L), minv.astype(L)
-    dt = np.asarray(time_step).astype(L)[:, None]
-    g = _grad(target, q)
-    for _ in range(n_steps):
-        p = p - (dt / 2) * g
-        q = q + dt * (p @ a.T)  # (M^-1 p) per row
-        g = _grad(target, q)
-        p = p - (dt / 2) * g
-    return q, p
-
-
-def _oracle_target(target, dim):
-    if target == "banana":
-        return otargets.Banana(dim, BANANA_B)
-    return {"std_gaussian": otargets.StdGaussian, "neal_funnel": otargets.NealFunnel}[target](dim)
-
-
-class _GivenInverse:
-    """A fixed dense metric given by the explicit float64 M^-1 the kernel multiplies with."""
-
-    kind = "dense"
-
-    def __init__(self, minv):
-        self.inv_array = minv
-
-    def inv_matvec(self, v):
-        return self.inv_array @ v
-
-    def sqrt_matvec(self, v):  # not used by the leapfrog
-        raise NotImplementedError
 
 
 # ------------------------------------------------------------------------------------------------
@@ -278,11 +193,6 @@ def _sample(n, sms, rng, extra=()):
     return np.unique(np.concatenate([first, last, pick, np.asarray(extra, dtype=np.int64)]))
 
 
-def _rel_err(x, ref):
-    """Per-chain max_i |x_i - ref_i| / max_i |ref_i| in units of 2^-52."""
-    return (np.abs(x.astype(L) - ref).max(1) / np.abs(ref).max(1) / L(ULP)).astype(np.float64)
-
-
 def _accumulation_roundings(dim):
     """Roundings of a position per drift inside K1 (documented deviation, DESIGN.md section 2):
     the drift accumulates into q itself, the DMMA accumulator, so q is rounded once per DMMA
@@ -291,18 +201,6 @@ def _accumulation_roundings(dim):
     (m16n8k16) DP / 16."""
     dp = 32 * -(-dim // 32)
     return dp // 8 + 1
-
-
-def _check_ratio(what, k1, orc, factor=1):
-    """K1's per-chain errors against `factor` x the float64 oracle's on the same chains: None or
-    the failure message, and the report line."""
-    kw, km, ow, om = k1.max(), k1.mean(), orc.max(), orc.mean()
-    report = f"{what} worst {kw:.2f}/{ow:.2f} mean {km:.3f}/{om:.3f}"
-    if kw > 4 * factor * ow + 8:
-        return f"{what}: K1 worst {kw:.2f} ulp vs {factor} x oracle worst {ow:.2f}", report
-    if km > 2 * factor * om + 2:
-        return f"{what}: K1 mean {km:.3f} ulp vs {factor} x oracle mean {om:.3f}", report
-    return None, report
 
 
 @pytest.mark.gpu
