@@ -265,6 +265,16 @@ struct UserRiemannianKernels {
 // the Riemannian part of a loaded user image (api_euclid.cu)
 const UserRiemannianKernels& user_riemannian_kernels(const void* handle);
 
+// Starts `kern` -- a library kernel, or a kernel of a loaded user image (a cudaKernel_t, which
+// only cudaLaunchKernel can start: a <<<>>> launch would call it as the kernel's host stub) --
+// with the argument types of the library's own instantiations
+template <class... P>
+inline void rm_start(void (*kern)(P...), unsigned blocks, int threads, size_t smem,
+                     cudaStream_t st, typename TypeTag<P>::type... args) {
+  void* argv[] = {&args...};
+  cudaLaunchKernel((const void*)kern, dim3(blocks), dim3(threads), argv, smem, st);
+}
+
 // Arguments of one implicit-integrator launch on a Riemannian system (leapfrog or midpoint steps;
 // zero steps evaluate the Hamiltonian only).  ws / ws_bytes: the caller's workspace, or NULL.
 struct ImplicitArgs {
@@ -305,5 +315,8 @@ int64_t dense_global_workspace_bytes(int64_t n_chains, int dim);
 bool dense_global_supported(int dim);
 int dense_global_implicit(const ImplicitArgs& a, bool hadamard);
 int dense_global_vector(const VectorArgs& a, bool velocity, bool hadamard);
+// the same launch plan for the kernel `kern` of a loaded user image (MB200_RMETRIC_USER_DENSE)
+int dense_global_implicit_image(const ImplicitArgs& a, const void* kern);
+int dense_global_vector_image(const VectorArgs& a, const void* kern);
 
 }  // namespace mb200

@@ -20,9 +20,12 @@ bool dense_global_supported(int dim) {
   return rm_smem_doubles(dim, RM_NMATS_GLOBAL) * sizeof(double) <= 227 * 1024;
 }
 
-template <template <class> class MetricT>
-static int dg_launch_implicit(const ImplicitArgs& a) {
-  auto kern = implicit_leapfrog_kernel<QuadraticRTarget, MetricT>;
+// The kernels this plan starts: a registry instantiation, or a kernel of a loaded user image (a
+// cudaKernel_t) with the same parameters
+using DgImplicitKernel = decltype(&implicit_leapfrog_kernel<QuadraticRTarget, GlobalDenseRank1>);
+using DgVectorKernel = decltype(&riemannian_velocity_kernel<QuadraticRTarget, GlobalDenseRank1>);
+
+static int dg_launch_implicit(DgImplicitKernel kern, const ImplicitArgs& a) {
   const size_t smem = rm_smem_doubles(a.dim, RM_NMATS_GLOBAL) * sizeof(double);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
@@ -32,18 +35,23 @@ static int dg_launch_implicit(const ImplicitArgs& a) {
   ModelArgs m = a.m;
   m.workspace = scratch.ptr;
   m.ws_stride = dg_workspace_doubles(a.dim);
-  kern<<<(unsigned)blocks, DG_THREADS, smem, a.st>>>(
-      a.q_in, a.p_in, a.q_out, a.p_out, a.dir, a.n, a.dim, a.eps, a.n_steps, m, a.fp_tol, a.fp_div,
-      a.fp_max, a.rev_tol, a.h_out, a.status, a.n_done, a.fp_iters, RM_NMATS_GLOBAL, 0, a.fp_solver);
+  rm_start(kern, (unsigned)blocks, DG_THREADS, smem, a.st, a.q_in, a.p_in, a.q_out, a.p_out, a.dir,
+           a.n, a.dim, a.eps, a.n_steps, m, a.fp_tol, a.fp_div, a.fp_max, a.rev_tol, a.h_out,
+           a.status, a.n_done, a.fp_iters, RM_NMATS_GLOBAL, 0, a.fp_solver);
   return check_launch("implicit_leapfrog_kernel (global dense metric)");
 }
 
 int dense_global_implicit(const ImplicitArgs& a, bool hadamard) {
-  return hadamard ? dg_launch_implicit<GlobalDenseHadamard>(a) : dg_launch_implicit<GlobalDenseRank1>(a);
+  return dg_launch_implicit(hadamard ? implicit_leapfrog_kernel<QuadraticRTarget, GlobalDenseHadamard>
+                                     : implicit_leapfrog_kernel<QuadraticRTarget, GlobalDenseRank1>,
+                            a);
 }
 
-template <template <class> class MetricT, bool VELOCITY>
-static int dg_launch_vec(const VectorArgs& a) {
+int dense_global_implicit_image(const ImplicitArgs& a, const void* kern) {
+  return dg_launch_implicit(reinterpret_cast<DgImplicitKernel>(kern), a);
+}
+
+static int dg_launch_vec(DgVectorKernel kern, const VectorArgs& a) {
   const size_t smem = rm_smem_doubles(a.dim, RM_NMATS_GLOBAL) * sizeof(double);
   const int blocks = dg_blocks(a.n);
   DgScratch scratch(nullptr, 0, (size_t)dense_global_workspace_bytes(a.n, a.dim), a.st);
@@ -51,19 +59,27 @@ static int dg_launch_vec(const VectorArgs& a) {
   ModelArgs m = a.m;
   m.workspace = scratch.ptr;
   m.ws_stride = dg_workspace_doubles(a.dim);
-  auto kern = riemannian_vector_kernel<QuadraticRTarget, MetricT, VELOCITY>();
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
-  kern<<<(unsigned)blocks, DG_THREADS, smem, a.st>>>(a.q, a.v, a.out, a.n, a.dim, m, a.status,
-                                                     RM_NMATS_GLOBAL);
+  rm_start(kern, (unsigned)blocks, DG_THREADS, smem, a.st, a.q, a.v, a.out, a.n, a.dim, m,
+           a.status, RM_NMATS_GLOBAL);
   return check_launch("riemannian vector kernel (global dense metric)");
 }
 
 // velocity: out = M(q)^-1 v ; else out = chol(M(q)) v
 int dense_global_vector(const VectorArgs& a, bool velocity, bool hadamard) {
   if (velocity)
-    return hadamard ? dg_launch_vec<GlobalDenseHadamard, true>(a) : dg_launch_vec<GlobalDenseRank1, true>(a);
-  return hadamard ? dg_launch_vec<GlobalDenseHadamard, false>(a) : dg_launch_vec<GlobalDenseRank1, false>(a);
+    return dg_launch_vec(hadamard ? riemannian_velocity_kernel<QuadraticRTarget, GlobalDenseHadamard>
+                                  : riemannian_velocity_kernel<QuadraticRTarget, GlobalDenseRank1>,
+                         a);
+  return dg_launch_vec(
+      hadamard ? riemannian_sample_momentum_kernel<QuadraticRTarget, GlobalDenseHadamard>
+               : riemannian_sample_momentum_kernel<QuadraticRTarget, GlobalDenseRank1>,
+      a);
+}
+
+int dense_global_vector_image(const VectorArgs& a, const void* kern) {
+  return dg_launch_vec(reinterpret_cast<DgVectorKernel>(kern), a);
 }
 
 }  // namespace mb200

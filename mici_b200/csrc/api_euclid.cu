@@ -416,9 +416,11 @@ int mb200_user_riemannian_load(const void* image, int64_t image_bytes, const cha
   if (!image || image_bytes <= 0 || !names || !handle)
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_names != 3) return fail(MB200_ERR_INVALID_ARG, "expected 3 kernel names, got %d", n_names);
-  if (rmetric_id != MB200_RMETRIC_USER_DIAGONAL && rmetric_id != MB200_RMETRIC_USER_SCALAR)
+  if (rmetric_id != MB200_RMETRIC_USER_DIAGONAL && rmetric_id != MB200_RMETRIC_USER_SCALAR &&
+      rmetric_id != MB200_RMETRIC_USER_DENSE)
     return fail(MB200_ERR_INVALID_ARG,
-                "rmetric_id must be MB200_RMETRIC_USER_DIAGONAL or MB200_RMETRIC_USER_SCALAR");
+                "rmetric_id must be MB200_RMETRIC_USER_DIAGONAL, MB200_RMETRIC_USER_SCALAR or "
+                "MB200_RMETRIC_USER_DENSE");
   return user_image_load(image, names, n_names, UserConstraintKernels{},
                          UserRiemannianKernels{rmetric_id, nullptr, nullptr, nullptr}, handle);
 }

@@ -68,15 +68,6 @@ static int rm_launch(Kernel kern, const char* name, RmOp op, int64_t n, int dim,
   return check_launch(name);
 }
 
-// Starts `kern` -- a library kernel, or a kernel of a loaded user image (a cudaKernel_t) -- with
-// the argument types of the library's own instantiations
-template <class... P>
-static void rm_start(void (*kern)(P...), unsigned blocks, int threads, size_t smem,
-                     cudaStream_t st, typename TypeTag<P>::type... args) {
-  void* argv[] = {&args...};
-  cudaLaunchKernel((const void*)kern, dim3(blocks), dim3(threads), argv, smem, st);
-}
-
 // Launch functors of the operations: `run<Target, MetricT>()` starts the operation's kernel for
 // that pair, `global(hadamard)` its global-workspace dense form (api_dense.cu), `image()` the
 // kernel of the loaded user image `user` (user_riemannian.cuh), planned from the traits the
@@ -109,6 +100,7 @@ struct ImplicitLaunch {
         });
   }
   int global(bool hadamard) const { return dense_global_implicit(a, hadamard); }
+  int image_global() const { return dense_global_implicit_image(a, user->implicit); }
 };
 
 template <RmOp OP>
@@ -135,6 +127,9 @@ struct VectorLaunch {
         });
   }
   int global(bool hadamard) const { return dense_global_vector(a, velocity, hadamard); }
+  int image_global() const {
+    return dense_global_vector_image(a, velocity ? user->velocity : user->momentum);
+  }
 };
 
 // The caller-provided workspace an implicit leapfrog of this model takes (the global-workspace
@@ -148,6 +143,7 @@ struct WorkspaceQuery {
   template <class Target, template <class> class MetricT>
   int run() const { return 0; }
   int image() const { return 0; }
+  int image_global() const { return 0; }
   int global(bool) const {
     *bytes = dense_global_workspace_bytes(n, dim);
     return 0;
@@ -171,7 +167,8 @@ static int run_on_target(int target_id, const L& l, const char* metric) {
 // Which kernel serves a Riemannian model, for every operation L::op: checks the model (the same
 // checks whatever the operation), picks the metric policy and the target, and hands them to `l`.
 // An operation's exclusions sit next to the route they restrict.  A loaded user image (l.user,
-// the *_user entry points) serves a user target with the image's own user metric.
+// the *_user entry points) serves a user target with the image's own user metric; a dense one
+// (MB200_RMETRIC_USER_DENSE) through the global-workspace launch plan, with its limits.
 template <class L>
 static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
   constexpr RmOp op = L::op;
@@ -182,7 +179,13 @@ static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
     if (m.rmetric_id != l.user->rmetric_id)
       return fail(MB200_ERR_INVALID_ARG, "rmetric_id %d does not match the user image's (%d)",
                   m.rmetric_id, l.user->rmetric_id);
-    return l.image();
+    if (l.user->rmetric_id != MB200_RMETRIC_USER_DENSE) return l.image();
+    if (op == RmOp::Midpoint)
+      return fail(MB200_ERR_UNSUPPORTED,
+                  "implicit midpoint is not available for the global-workspace dense metric");
+    if (!dense_global_supported(dim))
+      return fail(MB200_ERR_UNSUPPORTED, "dim %d: panel buffers exceed shared memory", dim);
+    return l.image_global();
   }
   // one per-chain D x D matrix (the rank-1 metric's Cholesky factor) fits in shared memory
   const bool fits = rm_smem_doubles(dim, 1) * sizeof(double) <= 227 * 1024;
@@ -376,10 +379,13 @@ int mb200_implicit_leapfrog_riemannian(
 // library then takes the scratch from the stream-ordered allocator for the duration of the call.
 int64_t mb200_implicit_workspace_bytes(int64_t n_chains, int32_t dim, const mb200_model* model) {
   if (!model || n_chains <= 0 || dim < 1) return 0;
-  // a user image's diagonal / scalar policies keep every per-chain vector in shared memory
+  // a user image's diagonal / scalar policies keep every per-chain vector in shared memory; its
+  // dense policy is the global-workspace one
   if (model->rmetric_id == MB200_RMETRIC_USER_DIAGONAL ||
       model->rmetric_id == MB200_RMETRIC_USER_SCALAR)
     return 0;
+  if (model->rmetric_id == MB200_RMETRIC_USER_DENSE)
+    return dense_global_supported(dim) ? dense_global_workspace_bytes(n_chains, dim) : 0;
   int64_t bytes = 0;
   rm_dispatch(to_args(model), dim, WorkspaceQuery{n_chains, dim, &bytes});
   return bytes;

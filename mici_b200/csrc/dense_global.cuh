@@ -25,6 +25,10 @@
 //   vjp_dense(q, V, out)  out_k = sum_ij V_ij dM_ij/dq_k for a dense symmetric V (here V = M^-1)
 //   vjp_rank1(q, w, out)  the same for V = -w w^T without forming it (the generic route that
 //                         forms -w w^T in the workspace and calls vjp_dense is kept: mp[3] != 0)
+// A registry model fills through entry(q, i, j), lower triangle only.  A model with its own
+// fill(k, q, M, ld) (the user model of user_riemannian.cuh) writes the whole n x n matrix; the
+// policy then checks every entry for finiteness and writes the identity padding itself.  A model
+// without vjp_rank1 always takes the generic route, and mp[3] is never read for it.
 #pragma once
 #include "riemannian.cuh"
 
@@ -600,6 +604,26 @@ struct HadamardModel {
 // ---------------------------------------------------------------------------------------------
 // Metric policy (same interface as the shared-memory policies of riemannian.cuh)
 // ---------------------------------------------------------------------------------------------
+
+// true for models that fill the whole matrix themselves (`fill`) instead of entry by entry
+template <class M, class = void>
+struct dg_model_fills {
+  static constexpr bool value = false;
+};
+template <class M>
+struct dg_model_fills<M, decltype(void(&M::fill))> {
+  static constexpr bool value = true;
+};
+// true for models with a rank-one VJP (`vjp_rank1`); the others take the generic route
+template <class M, class = void>
+struct dg_model_rank1 {
+  static constexpr bool value = false;
+};
+template <class M>
+struct dg_model_rank1<M, decltype(void(&M::vjp_rank1))> {
+  static constexpr bool value = true;
+};
+
 template <class Target, class Model>
 struct GlobalDenseMetricT {
   static constexpr bool SOFTABS = false;
@@ -613,8 +637,8 @@ struct GlobalDenseMetricT {
   const ModelArgs& margs;
 
   __device__ GlobalDenseMetricT(const Target& tt, const ModelArgs& m)
-      : t(tt), model(m, tt.dim), attached(false), have_inv(false), generic_rank1(m.mp[3] != 0.0),
-        margs(m) {}
+      : t(tt), model(m, tt.dim), attached(false), have_inv(false),
+        generic_rank1(!dg_model_rank1<Model>::value || m.mp[3] != 0.0), margs(m) {}
   __device__ void reset() {}
 
   __device__ int build(const Blk& k, RmWork& w, const double* q) {
@@ -623,6 +647,10 @@ struct GlobalDenseMetricT {
       attached = true;
     }
     have_inv = false;
+    if constexpr (dg_model_fills<Model>::value) return build_filled(k, q);
+    else return build_entries(k, q);
+  }
+  __device__ __forceinline__ int build_entries(const Blk& k, const double* q) {
     const int n = g.n, np = g.np;
     bool bad = false;
     // lower triangle only (the factorisation never reads above the diagonal blocks): one row
@@ -652,6 +680,30 @@ struct GlobalDenseMetricT {
       }
     }
     if (block_any(k, bad)) return MB200_STATUS_LINALG;  // "Array is not finite" (:211-215)
+    if (!dg_cholesky(k, g)) return MB200_STATUS_LINALG;
+    return 0;
+  }
+  // the model writes M(q) into rows / columns [0, n) of g.L; every one of those n x n entries is
+  // checked (both triangles: "Array is not finite", :211-215), then the rows and columns from n
+  // to np are reset to the identity and the lower triangle is factored
+  __device__ int build_filled(const Blk& k, const double* q) {
+    const int n = g.n, np = g.np;
+    double* const Lg = g.L;
+    RM_GLOBAL(Lg);
+    model.fill(k, q, Lg, np);
+    bool bad = false;
+    // one row per warp, lanes along the row
+    for (int i = k.warp; i < np; i += k.nwarp) {
+#pragma unroll 4
+      for (int j = k.lane; j < np; j += 32) {
+        if (i < n && j < n) {
+          if (!isfinite(Lg[(size_t)i * np + j])) bad = true;
+        } else {
+          Lg[(size_t)i * np + j] = (i == j) ? 1.0 : 0.0;
+        }
+      }
+    }
+    if (block_any(k, bad)) return MB200_STATUS_LINALG;
     if (!dg_cholesky(k, g)) return MB200_STATUS_LINALG;
     return 0;
   }
@@ -686,9 +738,11 @@ struct GlobalDenseMetricT {
   __device__ void vjp_grad_quad_inv(const Blk& k, RmWork& w, const double* q, const double* p,
                                     double* out) {
     dg_solve(k, g, p, w.ev, true, true);  // w = M^-1 p
-    if (!generic_rank1) {
-      model.vjp_rank1(k, q, w.ev, out);
-      return;
+    if constexpr (dg_model_rank1<Model>::value) {
+      if (!generic_rank1) {
+        model.vjp_rank1(k, q, w.ev, out);
+        return;
+      }
     }
     // generic route: materialise V = -w w^T in the workspace (X is free between inverses)
     const int n = g.n, np = g.np;
@@ -706,6 +760,7 @@ using GlobalDenseRank1 = GlobalDenseMetricT<Target, Rank1Model>;
 template <class Target>
 using GlobalDenseHadamard = GlobalDenseMetricT<Target, HadamardModel>;
 
+#ifndef __CUDACC_RTC__  // library self-test: kept out of the run-time compiled user images
 // Diagnostic kernel: factor / solve / invert arbitrary SPD matrices (one CTA per matrix) so that
 // the blocked routines can be checked against numpy.linalg directly (tests/test_parity_gpu.py).
 static __global__ void __launch_bounds__(DG_THREADS)
@@ -750,5 +805,6 @@ static __global__ void __launch_bounds__(DG_THREADS)
     if (k.tid == 0) status[mi] = ok ? 0 : MB200_STATUS_LINALG;
   }
 }
+#endif
 
 }  // namespace mb200

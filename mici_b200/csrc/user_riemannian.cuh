@@ -1,6 +1,7 @@
-// User-written targets and metrics on the diagonal and scalar Riemannian systems, compiled at run
-// time by NVRTC (mici_b200/jit.py) together with the implicit-integrator, velocity and
-// momentum-refresh kernels of riemannian.cuh (K9).
+// User-written targets and metrics on the diagonal, scalar and dense Riemannian systems, compiled
+// at run time by NVRTC (mici_b200/jit.py) together with the implicit-integrator, velocity and
+// momentum-refresh kernels of riemannian.cuh (K9) or, for a dense metric, of the global-workspace
+// dense policy of dense_global.cuh (K2g, K13).
 //
 // Besides neg_log_dens and grad_neg_log_dens (user_target.cuh), the user writes one pair:
 //
@@ -12,6 +13,12 @@
 //   __device__ double metric_scalar(const mb200::Chain& c);        // s(q), the same on every lane
 //   __device__ void vjp_metric_scalar(const mb200::Chain& c, double w, double* out);
 //                                                          // out[j] = w ds / dq_j
+//   // DenseRiemannianMetricSystem: M(q) dense, positive definite
+//   __device__ void metric_dense(const mb200::CtaChain& c, double* M, int ld);
+//                                          // M[i * ld + j] = M_ij(q) for all 0 <= i, j < dim
+//   __device__ void vjp_metric_dense(const mb200::CtaChain& c, const double* V, int ld,
+//                                    double* out);
+//           // out[k] = sum_ij V[i * ld + j] dM_ij / dq_k, V symmetric, every out[k], k < dim
 //
 // The rules of user_target.cuh apply to every function.  Inside the metric functions c.params
 // and c.aux are the metric's own (mb200_model.rmetric_params / rmetric_aux); c.q is the position.
@@ -20,15 +27,37 @@
 // call or in the same call before a c.sum().  A d_i or s that is not positive (or NaN) fails as
 // with the registry metrics: LinAlgError outside a fixed-point solve, ConvergenceError inside one.
 //
-// The host defines MB200_USER_DIAGONAL_METRIC or MB200_USER_SCALAR_METRIC and puts
-// MB200_USER_METRIC_FUNCTIONS after the user sources: that binds the pair to the policies, so a
-// missing function is reported at the end of the user's own source.
+// The dense metric runs on the global-workspace dense policy: one 256-thread CTA per chain, the
+// D x D matrices in a per-CTA global workspace.  Its two functions are called by the WHOLE CTA
+// and see the chain through mb200::CtaChain: c.lane in [0, c.n_lanes), c.n_lanes == 256, and
+// c.sum(), a CTA all-reduce in a fixed order that every thread must reach.  Each call sits
+// between two __syncthreads(); M and V are in global memory (L2), q and out in shared memory.
+// The intended style is `for (int i = c.lane; i < c.dim; i += c.n_lanes)` over rows, or over the
+// D^2 entries.  The target keeps its warp contract: warp 0 alone calls neg_log_dens /
+// grad_neg_log_dens while the other warps wait, so one CudaTarget source runs on every system.
+// As in the reference (DenseRiemannianMetricSystem, numpy.linalg.cholesky):
+//  - every entry of the dim x dim matrix, both triangles, must be finite; one that is not is a
+//    LinAlgError;
+//  - only the lower triangle is factored (the upper one is never read);
+//  - a pivot that is not positive is a LinAlgError;
+//  - inside a fixed-point solve both failures are a ConvergenceError.
+// The policy, not the user, writes the identity padding of the rows and columns from dim to the
+// padded dimension (a multiple of 32) after every fill.  dim <= 576.
+//
+// The host defines exactly one of MB200_USER_DIAGONAL_METRIC, MB200_USER_SCALAR_METRIC and
+// MB200_USER_DENSE_METRIC and puts MB200_USER_METRIC_FUNCTIONS after the user sources: that binds
+// the pair to the policies, so a missing function is reported at the end of the user's own source.
 #pragma once
 #include "user_target.cuh"
 #include "riemannian.cuh"
 
-#if defined(MB200_USER_DIAGONAL_METRIC) == defined(MB200_USER_SCALAR_METRIC)
-#error "define exactly one of MB200_USER_DIAGONAL_METRIC and MB200_USER_SCALAR_METRIC"
+#if defined(MB200_USER_DIAGONAL_METRIC) + defined(MB200_USER_SCALAR_METRIC) + \
+        defined(MB200_USER_DENSE_METRIC) != 1
+#error "define exactly one of MB200_USER_DIAGONAL_METRIC, MB200_USER_SCALAR_METRIC and MB200_USER_DENSE_METRIC"
+#endif
+
+#ifdef MB200_USER_DENSE_METRIC
+#include "dense_global.cuh"
 #endif
 
 namespace mb200 {
@@ -127,6 +156,83 @@ using UserDiagonalMetric = DiagonalMetric<Target, UserDiagModel<>>;
 template <class Target>
 using UserScalarMetric = ScalarMetric<Target, UserScalarModel<>>;
 
+#ifdef MB200_USER_DENSE_METRIC
+// What a dense metric function sees of one chain: the whole CTA
+struct CtaChain {
+  int dim;
+  int lane;                         // 0 .. n_lanes - 1: the thread of the CTA
+  int n_lanes;                      // 256
+  const double* q;                  // the whole position vector [dim], shared memory
+  double params[MB200_MAX_PARAMS];  // mb200_model.rmetric_params
+  const double* aux;                // mb200_model.rmetric_aux (device array) or NULL
+  Blk blk;
+  // CTA all-reduce in a fixed order (warp butterflies, then the warp totals in order): every
+  // thread gets the same value
+  __device__ __forceinline__ double sum(double x) const { return block_sum(blk, x); }
+};
+
+// The target's warp contract on the dense policy's 256-thread CTA: warp 0 calls the user
+// functions, the other warps wait at the barrier; the value of l reaches every thread through
+// shared memory (the reduction scratch's slot 32, which block_sum / block_nanmax never use)
+struct UserRTargetCta : UserRTarget {
+  __device__ UserRTargetCta(const ModelArgs& m, int d) : UserRTarget(m, d) {}
+  __device__ double nld(const Blk& k, const double* q) const {
+    __syncthreads();
+    if (k.warp == 0) {
+      const double v = u.nld(q, dim, k.lane);
+      if (k.lane == 0) k.red[32] = v;
+    }
+    __syncthreads();
+    return k.red[32];
+  }
+  __device__ void grad(const Blk& k, const double* q, double* g) const {
+    __syncthreads();
+    if (k.warp == 0) u.grad(q, dim, k.lane, g);
+    __syncthreads();
+  }
+};
+
+// GlobalDenseMetricT's model interface over metric_dense / vjp_metric_dense: fill and the dense
+// VJP, no entry and no rank-one VJP (the policy forms V = -w w^T for the generic route)
+template <class F = UserMetricFunctions>
+struct UserDenseModel {
+  double mp[MB200_MAX_PARAMS];
+  const double* maux;
+  int dim;
+  __device__ UserDenseModel(const ModelArgs& m, int d) : maux(m.maux), dim(d) {
+#pragma unroll
+    for (int i = 0; i < MB200_MAX_PARAMS; ++i) mp[i] = m.mp[i];
+  }
+  __device__ __forceinline__ CtaChain chain(const Blk& k, const double* q) const {
+    CtaChain c;
+    c.dim = dim;
+    c.lane = k.tid;
+    c.n_lanes = k.nthr;
+    c.q = q;
+#pragma unroll
+    for (int i = 0; i < MB200_MAX_PARAMS; ++i) c.params[i] = mp[i];
+    c.aux = maux;
+    c.blk = k;
+    return c;
+  }
+  __device__ void fill(const Blk& k, const double* q, double* M, int ld) const {
+    __syncthreads();
+    F::dense(chain(k, q), M, ld);
+    __syncthreads();
+  }
+  __device__ void vjp_dense(const Blk& k, const double* q, const double* V, int ld,
+                            double* out) const {
+    __syncthreads();
+    F::vjp(chain(k, q), V, ld, out);
+    __syncthreads();
+  }
+};
+
+template <class Target>
+using UserDenseMetric = GlobalDenseMetricT<Target, UserDenseModel<>>;
+static_assert(DG_THREADS == 256, "the dense user contract is per 256-thread CTA");
+#endif
+
 template <class P>
 constexpr bool user_policy_traits_match() {
   using H = UserRPolicyTraits<UserRTarget>;
@@ -148,6 +254,17 @@ static_assert(user_policy_traits_match<DiagonalMetric<UserRTarget, QuadraticDiag
     static __device__ __forceinline__ void vjp(const mb200::Chain& c, const double* w,          \
                                                double* out) {                                   \
       vjp_metric_diagonal(c, w, out);                                                           \
+    }                                                                                           \
+  };
+#elif defined(MB200_USER_DENSE_METRIC)
+#define MB200_USER_METRIC_FUNCTIONS                                                             \
+  struct mb200::UserMetricFunctions {                                                           \
+    static __device__ __forceinline__ void dense(const mb200::CtaChain& c, double* M, int ld) { \
+      metric_dense(c, M, ld);                                                                   \
+    }                                                                                           \
+    static __device__ __forceinline__ void vjp(const mb200::CtaChain& c, const double* V,       \
+                                               int ld, double* out) {                           \
+      vjp_metric_dense(c, V, ld, out);                                                          \
     }                                                                                           \
   };
 #else

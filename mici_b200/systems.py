@@ -30,6 +30,7 @@ from .errors import LinAlgError
 from .solvers import solve_projection_onto_manifold_newton
 from .targets import (
     RMETRIC_SOFTABS,
+    CudaDenseMetric,
     CudaDiagonalMetric,
     CudaRiemannianPair,
     CudaScalarMetric,
@@ -735,16 +736,27 @@ class DenseRiemannianMetricSystem(RiemannianMetricSystem):
     metric is factorised (Cholesky), inverted explicitly and differentiated through the model's
     VJP as the reference does (matrices.py:1161-1188, systems.py:1381-1399): in shared memory
     for D <= 160, in a per-CTA global workspace with DMMA-blocked routines beyond
-    (csrc/dense_global.cuh)."""
+    (csrc/dense_global.cuh).
+
+    ``metric_func`` may also be a user-written ``mici_b200.targets.CudaDenseMetric`` with an
+    unconstrained ``CudaTarget`` (``dim <= 576``): it runs on the global-workspace policy at every
+    dimension, without the implicit midpoint integrator."""
+
+    # the largest dimension whose panel buffers fit in shared memory (dense_global_supported)
+    MAX_USER_DIM = 576
 
     def __init__(self, neg_log_dens, metric_func, *, vjp_metric_func=None,
                  grad_neg_log_dens=None, backend=None):
+        self._accept_user_metric(neg_log_dens, metric_func, CudaDenseMetric)
         super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
-        if not isinstance(metric_func, (Rank1Metric, HadamardMetric)):
+        if not isinstance(metric_func, (Rank1Metric, HadamardMetric, CudaDenseMetric)):
             raise TypeError("`metric_func` must be a registered metric model "
-                            "(Rank1Metric or HadamardMetric).")
+                            "(Rank1Metric or HadamardMetric) or a CudaDenseMetric.")
         if vjp_metric_func is not None:
             raise ValueError("The metric VJP is fused into the kernels.")
+        if isinstance(metric_func, CudaDenseMetric) and neg_log_dens.dim > self.MAX_USER_DIM:
+            raise ValueError(f"A CudaDenseMetric needs dim <= {self.MAX_USER_DIM}, "
+                             f"got {neg_log_dens.dim}.")
         self.metric_model = metric_func
         self._rmetric_id = metric_func.rmetric_id
         self._rmetric_params = metric_func.params

@@ -31,6 +31,7 @@ RMETRIC_SCALAR_QUADRATIC = 5
 RMETRIC_CHOL_QUADRATIC = 6
 RMETRIC_USER_DIAGONAL = 32  # MB200_RMETRIC_USER_DIAGONAL: CudaDiagonalMetric
 RMETRIC_USER_SCALAR = 33  # MB200_RMETRIC_USER_SCALAR: CudaScalarMetric
+RMETRIC_USER_DENSE = 34  # MB200_RMETRIC_USER_DENSE: CudaDenseMetric
 
 
 class Target:
@@ -237,7 +238,7 @@ class CudaTarget(Target):
 
 
 class _CudaMetric:
-    """A user-written diagonal or scalar metric (contract: ``mici_b200/csrc/user_riemannian.cuh``):
+    """A user-written diagonal, scalar or dense metric (contract: ``mici_b200/csrc/user_riemannian.cuh``):
     CUDA C++ source, at most 8 ``params`` (``c.params`` inside the metric functions) and an
     optional ``aux`` array (``c.aux``).  It runs with a ``CudaTarget`` only, compiled with it into
     one image; like the target it holds only source, params and aux."""
@@ -294,6 +295,26 @@ class CudaScalarMetric(_CudaMetric):
 
     kind = "scalar"
     rmetric_id = RMETRIC_USER_SCALAR
+
+
+class CudaDenseMetric(_CudaMetric):
+    """A user-written dense metric M(q), positive definite, for ``DenseRiemannianMetricSystem``:
+    CUDA C++ source defining
+
+        __device__ void metric_dense(const mb200::CtaChain& c, double* M, int ld);
+        __device__ void vjp_metric_dense(const mb200::CtaChain& c, const double* V, int ld,
+                                         double* out);
+
+    with ``M[i * ld + j] = M_ij(q)`` for all ``i, j < dim`` and ``out[k] = sum_ij V[i * ld + j]
+    dM_ij/dq_k`` for a symmetric ``V``, every ``out[k], k < dim`` written.  Both functions are
+    called by the whole 256-thread CTA of the chain (``c.lane`` in ``[0, c.n_lanes)``, ``c.sum()``
+    a CTA all-reduce), not by one warp; the target keeps its warp contract.  Every entry of the
+    matrix must be finite and only its lower triangle is factored, as ``numpy.linalg.cholesky``
+    does; a failure is a ``LinAlgError`` outside a fixed-point solve and a ``ConvergenceError``
+    inside one.  ``dim <= 576``.  Contract: ``mici_b200/csrc/user_riemannian.cuh``."""
+
+    kind = "dense"
+    rmetric_id = RMETRIC_USER_DENSE
 
 
 class CudaRiemannianPair:
