@@ -95,12 +95,13 @@ extern "C" {
 /* Cholesky-factored metric M = L L^T given by its lower factor (CholeskyFactoredRiemannianMetricSystem,
  * systems.py:1574-1653); targets: std-Gaussian, banana, funnel, quadratic */
 #define MB200_RMETRIC_CHOL_QUADRATIC 6 /* L(q) = L0 + c tril(q q^T);  aux: L0 [dim*dim] row-major, upper triangle zero (never read), params: c */
-/* user-written diagonal / scalar / dense metrics compiled at run time with a user target
+/* user-written diagonal / scalar / dense / Cholesky-factored metrics compiled at run time with a user target
  * (mb200_user_riemannian_load); only the Riemannian *_user entry points accept them, every registry
  * entry point rejects them as an unknown rmetric_id.  params / aux: the metric's own */
 #define MB200_RMETRIC_USER_DIAGONAL 32
 #define MB200_RMETRIC_USER_SCALAR 33
 #define MB200_RMETRIC_USER_DENSE 34 /* global-workspace dense policy: dim <= 576, no implicit midpoint */
+#define MB200_RMETRIC_USER_CHOLESKY 35 /* triangular-factored policy: dim <= 1016 */
 
 /* fixed-point solvers fused into the implicit integrators (solvers.py:47-94, 97-154) */
 #define MB200_FP_SOLVER_DIRECT 0
@@ -468,14 +469,16 @@ int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_o
                              int32_t* status, void* stream);
 
 /*
- * User-written targets and metrics on the diagonal, scalar and dense Riemannian systems
- * (mici_b200/csrc/user_riemannian.cuh): a user target and a user diagonal, scalar or dense metric
- * compiled at run time, by NVRTC, together with the Riemannian kernels of the compact policies or
- * of the global-workspace dense policy (mici_b200/csrc/dense_global.cuh).
+ * User-written targets and metrics on the diagonal, scalar, dense and Cholesky-factored Riemannian
+ * systems (mici_b200/csrc/user_riemannian.cuh): a user target and a user diagonal, scalar, dense
+ * or Cholesky-factored metric compiled at run time, by NVRTC, together with the Riemannian kernels
+ * of the compact policies, of the triangular-factored policy or of the global-workspace dense
+ * policy (mici_b200/csrc/dense_global.cuh).
  *  - mb200_user_riemannian_load: loads a CUBIN `image` of `n_names` = 3 kernels, with
  *    T = UserRTarget and M = UserDiagonalMetric (rmetric_id MB200_RMETRIC_USER_DIAGONAL) or
  *    UserScalarMetric (MB200_RMETRIC_USER_SCALAR), or T = UserRTargetCta and M = UserDenseMetric
- *    (MB200_RMETRIC_USER_DENSE): implicit_leapfrog_kernel<T, M>,
+ *    (MB200_RMETRIC_USER_DENSE) or UserCholeskyMetric (MB200_RMETRIC_USER_CHOLESKY):
+ *    implicit_leapfrog_kernel<T, M>,
  *    riemannian_velocity_kernel<T, M>, riemannian_sample_momentum_kernel<T, M>.  The handle is
  *    released by mb200_user_target_unload.  It serves only the Riemannian *_user entry points;
  *    the Euclidean and constrained ones refuse it, and these refuse every other handle.
@@ -491,6 +494,12 @@ int mb200_dh_dmom_riemannian(const double* pos, const double* mom, double* vel_o
  *    bytes; less or NULL: a stream-ordered allocation for the call).  Refused before any launch:
  *    the implicit midpoint (MB200_ERR_UNSUPPORTED, as for the registry Hadamard metric) and
  *    dim > 576 (MB200_ERR_UNSUPPORTED).
+ *  - A Cholesky-factored image runs on the launch plan of the registry's Cholesky-factored metric
+ *    with two per-chain matrices (the factor L and the matrix V the policy differentiates): one
+ *    256-thread CTA per chain, both matrices in shared memory up to dim 112 and in a per-CTA
+ *    global workspace that the library allocates itself (stream-ordered) beyond;
+ *    mb200_implicit_workspace_bytes returns 0.  Both integrators are supported.  dim > 1016, where
+ *    the per-chain vectors exceed shared memory, is MB200_ERR_UNSUPPORTED before any launch.
  */
 int mb200_user_riemannian_load(const void* image, int64_t image_bytes, const char* const* names,
                                int32_t n_names, int32_t rmetric_id, void** handle);

@@ -417,10 +417,10 @@ int mb200_user_riemannian_load(const void* image, int64_t image_bytes, const cha
     return fail(MB200_ERR_INVALID_ARG, "null pointer argument");
   if (n_names != 3) return fail(MB200_ERR_INVALID_ARG, "expected 3 kernel names, got %d", n_names);
   if (rmetric_id != MB200_RMETRIC_USER_DIAGONAL && rmetric_id != MB200_RMETRIC_USER_SCALAR &&
-      rmetric_id != MB200_RMETRIC_USER_DENSE)
+      rmetric_id != MB200_RMETRIC_USER_DENSE && rmetric_id != MB200_RMETRIC_USER_CHOLESKY)
     return fail(MB200_ERR_INVALID_ARG,
-                "rmetric_id must be MB200_RMETRIC_USER_DIAGONAL, MB200_RMETRIC_USER_SCALAR or "
-                "MB200_RMETRIC_USER_DENSE");
+                "rmetric_id must be MB200_RMETRIC_USER_DIAGONAL, MB200_RMETRIC_USER_SCALAR, "
+                "MB200_RMETRIC_USER_DENSE or MB200_RMETRIC_USER_CHOLESKY");
   return user_image_load(image, names, n_names, UserConstraintKernels{},
                          UserRiemannianKernels{rmetric_id, nullptr, nullptr, nullptr}, handle);
 }

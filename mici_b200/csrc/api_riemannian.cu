@@ -69,9 +69,9 @@ static int rm_launch(Kernel kern, const char* name, RmOp op, int64_t n, int dim,
 }
 
 // Launch functors of the operations: `run<Target, MetricT>()` starts the operation's kernel for
-// that pair, `global(hadamard)` its global-workspace dense form (api_dense.cu), `image()` the
-// kernel of the loaded user image `user` (user_riemannian.cuh), planned from the traits the
-// image's policies share with the host (UserRPolicyTraits)
+// that pair, `global(hadamard)` its global-workspace dense form (api_dense.cu), `image<Traits>()`
+// the kernel of the loaded user image `user` (user_riemannian.cuh), planned from the traits the
+// image's policy shares with the host (UserRPolicyTraits, UserRCholPolicyTraits)
 using ImplicitKernel = decltype(&implicit_leapfrog_kernel<StdGaussianRTarget, QuadraticDiagonalMetric>);
 using VectorKernel = decltype(&riemannian_velocity_kernel<StdGaussianRTarget, QuadraticDiagonalMetric>);
 
@@ -84,9 +84,9 @@ struct ImplicitLaunch {
   int run() const {
     return launch<Target, MetricT>(implicit_leapfrog_kernel<Target, MetricT>);
   }
+  template <template <class> class Traits>
   int image() const {
-    return launch<UserRTargetTraits, UserRPolicyTraits>(
-        reinterpret_cast<ImplicitKernel>(user->implicit));
+    return launch<UserRTargetTraits, Traits>(reinterpret_cast<ImplicitKernel>(user->implicit));
   }
   template <class Target, template <class> class MetricT>
   int launch(ImplicitKernel kern) const {
@@ -113,8 +113,9 @@ struct VectorLaunch {
   int run() const {
     return launch<Target, MetricT>(riemannian_vector_kernel<Target, MetricT, velocity>());
   }
+  template <template <class> class Traits>
   int image() const {
-    return launch<UserRTargetTraits, UserRPolicyTraits>(
+    return launch<UserRTargetTraits, Traits>(
         reinterpret_cast<VectorKernel>(velocity ? user->velocity : user->momentum));
   }
   template <class Target, template <class> class MetricT>
@@ -142,6 +143,7 @@ struct WorkspaceQuery {
   const UserRiemannianKernels* user = nullptr;
   template <class Target, template <class> class MetricT>
   int run() const { return 0; }
+  template <template <class> class>
   int image() const { return 0; }
   int image_global() const { return 0; }
   int global(bool) const {
@@ -167,8 +169,10 @@ static int run_on_target(int target_id, const L& l, const char* metric) {
 // Which kernel serves a Riemannian model, for every operation L::op: checks the model (the same
 // checks whatever the operation), picks the metric policy and the target, and hands them to `l`.
 // An operation's exclusions sit next to the route they restrict.  A loaded user image (l.user,
-// the *_user entry points) serves a user target with the image's own user metric; a dense one
-// (MB200_RMETRIC_USER_DENSE) through the global-workspace launch plan, with its limits.
+// the *_user entry points) serves a user target with the image's own user metric, planned from
+// the host traits of its policy: the compact ones (diagonal, scalar), the triangular-factored one
+// (MB200_RMETRIC_USER_CHOLESKY: 256-thread CTAs, the factor and V per chain), or, for a dense
+// one (MB200_RMETRIC_USER_DENSE), the global-workspace launch plan with its limits.
 template <class L>
 static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
   constexpr RmOp op = L::op;
@@ -179,7 +183,10 @@ static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
     if (m.rmetric_id != l.user->rmetric_id)
       return fail(MB200_ERR_INVALID_ARG, "rmetric_id %d does not match the user image's (%d)",
                   m.rmetric_id, l.user->rmetric_id);
-    if (l.user->rmetric_id != MB200_RMETRIC_USER_DENSE) return l.image();
+    if (l.user->rmetric_id == MB200_RMETRIC_USER_CHOLESKY)
+      return l.template image<UserRCholPolicyTraits>();
+    if (l.user->rmetric_id != MB200_RMETRIC_USER_DENSE)
+      return l.template image<UserRPolicyTraits>();
     if (op == RmOp::Midpoint)
       return fail(MB200_ERR_UNSUPPORTED,
                   "implicit midpoint is not available for the global-workspace dense metric");
@@ -379,10 +386,12 @@ int mb200_implicit_leapfrog_riemannian(
 // library then takes the scratch from the stream-ordered allocator for the duration of the call.
 int64_t mb200_implicit_workspace_bytes(int64_t n_chains, int32_t dim, const mb200_model* model) {
   if (!model || n_chains <= 0 || dim < 1) return 0;
-  // a user image's diagonal / scalar policies keep every per-chain vector in shared memory; its
-  // dense policy is the global-workspace one
+  // a user image's diagonal / scalar policies keep every per-chain vector in shared memory, its
+  // Cholesky-factored policy allocates its per-CTA workspace itself (as the registry one does);
+  // its dense policy is the global-workspace one
   if (model->rmetric_id == MB200_RMETRIC_USER_DIAGONAL ||
-      model->rmetric_id == MB200_RMETRIC_USER_SCALAR)
+      model->rmetric_id == MB200_RMETRIC_USER_SCALAR ||
+      model->rmetric_id == MB200_RMETRIC_USER_CHOLESKY)
     return 0;
   if (model->rmetric_id == MB200_RMETRIC_USER_DENSE)
     return dense_global_supported(dim) ? dense_global_workspace_bytes(n_chains, dim) : 0;

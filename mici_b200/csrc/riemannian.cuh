@@ -1653,6 +1653,19 @@ struct QuadraticCholModel {
   }
 };
 
+// true for Cholesky models that differentiate a lower-triangular V itself (`static constexpr bool
+// DENSE_VJP = true` and vjp_tril(k, q, V, ld, out): out[k] = sum_{j<=i} V_ij dL_ij/dq_k, the
+// user models of user_riemannian.cuh); the policy then forms V in a second per-chain matrix, w.M2.
+// The registry model declares nothing and takes the structured VJPs vjp_diag / vjp_outer.
+template <class M, class = void>
+struct chol_dense_vjp {
+  static constexpr bool value = false;
+};
+template <class M>
+struct chol_dense_vjp<M, decltype(void(M::DENSE_VJP))> {
+  static constexpr bool value = M::DENSE_VJP;
+};
+
 // TriangularFactoredPositiveDefiniteMatrix(L, factor_is_lower=True):
 //   log|M| = 2 sum log|L_ii|                          (matrices.py:982-984, 850-852)
 //   M^-1 v = L^-T (L^-1 v), no inverse formed          (:1110-1111, 897-912)
@@ -1663,14 +1676,21 @@ struct QuadraticCholModel {
 // (ExplicitArrayMatrix, :207-215); a zero or negative diagonal entry is accepted, as by the
 // reference: a zero pivot surfaces through IEEE arithmetic in the solves (-> ConvergenceError
 // inside a fixed-point solve) and through singular() in the velocity and energy evaluations.
+// A DENSE_VJP model (chol_dense_vjp) gets the two gradients as lower-triangular matrices V in w.M2
+// (its strict upper triangle is never written), one vjp_tril call each, as the reference's
+// vjp_metric_chol_func(q)(V) does.
 template <class Target, class Model>
 struct CholeskyFactoredMetric {
   static constexpr bool SOFTABS = false;
   static constexpr bool CAN_BE_SINGULAR = true;
-  static constexpr int N_MATS = 1;          // the factor [dim x (dim + 1)]
-  static constexpr int WORKSPACE_MATS = 1;  // ... in the per-CTA global workspace beyond ~150
+  // the factor [dim x (dim + 1)], and V for a DENSE_VJP model; in the per-CTA global workspace
+  // beyond D ~ 150 (one matrix) or D ~ 113 (two)
+  static constexpr int N_MATS = chol_dense_vjp<Model>::value ? 2 : 1;
+  static constexpr int WORKSPACE_MATS = N_MATS;
   static constexpr int THREADS = MB200_RM_CHOL_THREADS;
-  static constexpr int MIN_BLOCKS = 65536 / 128 / THREADS;  // <= 128 registers
+  // <= 128 registers; a DENSE_VJP model: up to 255, since the user functions and the target's
+  // parameters would not fit beside the policy's state without spilling
+  static constexpr int MIN_BLOCKS = chol_dense_vjp<Model>::value ? 1 : 65536 / 128 / THREADS;
   const Target& t;
   Model model;
   __device__ CholeskyFactoredMetric(const Target& tt, const ModelArgs& m) : t(tt), model(m, tt.dim) {}
@@ -1704,28 +1724,59 @@ struct CholeskyFactoredMetric {
     __syncthreads();
     return true;
   }
-  // d = 2 / diag L in w.ev
+  // d = 2 / diag L in w.ev; a DENSE_VJP model: V = diag(d) in w.M2, strict lower triangle zero
   __device__ void vjp_grad_log_abs_det(const Blk& k, RmWork& w, const double* q, double* out) {
-    for (int i = k.tid; i < w.dim; i += k.nthr) w.ev[i] = 2.0 / w.M1[i * w.ld + i];
-    __syncthreads();
-    model.vjp_diag(k, q, w.ev, out);
+    if constexpr (chol_dense_vjp<Model>::value) {
+      const int ld = w.ld;
+      for (int i = k.warp; i < w.dim; i += k.nwarp)  // one row per warp: coalesced
+        for (int j = k.lane; j <= i; j += 32)
+          w.M2[i * ld + j] = j == i ? 2.0 / w.M1[i * ld + i] : 0.0;
+      __syncthreads();
+      model.vjp_tril(k, q, w.M2, ld, out);
+    } else {
+      for (int i = k.tid; i < w.dim; i += k.nthr) w.ev[i] = 2.0 / w.M1[i * w.ld + i];
+      __syncthreads();
+      model.vjp_diag(k, q, w.ev, out);
+    }
     __syncthreads();
   }
   // b = L^-1 p in w.lam (computed once: M^-1 p = L^-T b continues from it), a = M^-1 p in w.ev;
-  // scan scratch w.sa, w.gsa
+  // scan scratch w.sa, w.gsa.  A DENSE_VJP model: V = tril(-2 a b^T) in w.M2
   __device__ void vjp_grad_quad_inv(const Blk& k, RmWork& w, const double* q, const double* p,
                                     double* out) {
     cholesky_forward(k, w.M1, w.dim, w.ld, p, w.lam);
     for (int i = k.tid; i < w.dim; i += k.nthr) w.ev[i] = w.lam[i];
     __syncthreads();
     cholesky_back(k, w.M1, w.dim, w.ld, w.ev);
-    model.vjp_outer(k, q, -2.0, w.ev, w.lam, w.sa, w.gsa, out);
+    if constexpr (chol_dense_vjp<Model>::value) {
+      const int ld = w.ld;
+      for (int i = k.warp; i < w.dim; i += k.nwarp) {
+        const double a = w.ev[i];
+        for (int j = k.lane; j <= i; j += 32) w.M2[i * ld + j] = -2.0 * (a * w.lam[j]);
+      }
+      __syncthreads();
+      model.vjp_tril(k, q, w.M2, ld, out);
+    } else {
+      model.vjp_outer(k, q, -2.0, w.ev, w.lam, w.sa, w.gsa, out);
+    }
     __syncthreads();
   }
 };
 
 template <class Target>
 using QuadraticCholeskyMetric = CholeskyFactoredMetric<Target, QuadraticCholModel>;
+
+// What rm_launch reads of a user image's Cholesky-factored policy (CholeskyFactoredMetric over the
+// user functions of user_riemannian.cuh, which checks these values): the factor and V per chain
+template <class>
+struct UserRCholPolicyTraits {
+  static constexpr bool SOFTABS = false;
+  static constexpr bool COMPACT = false;
+  static constexpr int N_MATS = 2;
+  static constexpr int WORKSPACE_MATS = 2;
+  static constexpr int MIN_BLOCKS = 1;
+  static constexpr int THREADS = MB200_RM_CHOL_THREADS;
+};
 
 // ---------------------------------------------------------------------------------------------
 // K4: solve_fixed_point_direct (solvers.py:47-94) for one chain, block-cooperative.

@@ -1,7 +1,7 @@
-// User-written targets and metrics on the diagonal, scalar and dense Riemannian systems, compiled
-// at run time by NVRTC (mici_b200/jit.py) together with the implicit-integrator, velocity and
-// momentum-refresh kernels of riemannian.cuh (K9) or, for a dense metric, of the global-workspace
-// dense policy of dense_global.cuh (K2g, K13).
+// User-written targets and metrics on the diagonal, scalar, dense and Cholesky-factored Riemannian
+// systems, compiled at run time by NVRTC (mici_b200/jit.py) together with the implicit-integrator,
+// velocity and momentum-refresh kernels of riemannian.cuh (K9, K10, K14) or, for a dense metric, of
+// the global-workspace dense policy of dense_global.cuh (K2g, K13).
 //
 // Besides neg_log_dens and grad_neg_log_dens (user_target.cuh), the user writes one pair:
 //
@@ -19,6 +19,13 @@
 //   __device__ void vjp_metric_dense(const mb200::CtaChain& c, const double* V, int ld,
 //                                    double* out);
 //           // out[k] = sum_ij V[i * ld + j] dM_ij / dq_k, V symmetric, every out[k], k < dim
+//   // CholeskyFactoredRiemannianMetricSystem: M(q) = L(q) L(q)^T, L lower triangular
+//   __device__ void metric_chol(const mb200::CtaChain& c, double* L, int ld);
+//                  // L[i * ld + j] = L_ij(q) for 0 <= j <= i < dim; the upper triangle is never read
+//   __device__ void vjp_metric_chol(const mb200::CtaChain& c, const double* V, int ld,
+//                                   double* out);
+//           // out[k] = sum_{j <= i} V[i * ld + j] dL_ij / dq_k, every out[k], k < dim; V is lower
+//           // triangular and its entries above the diagonal must not be read
 //
 // The rules of user_target.cuh apply to every function.  Inside the metric functions c.params
 // and c.aux are the metric's own (mb200_model.rmetric_params / rmetric_aux); c.q is the position.
@@ -44,16 +51,30 @@
 // The policy, not the user, writes the identity padding of the rows and columns from dim to the
 // padded dimension (a multiple of 32) after every fill.  dim <= 576.
 //
-// The host defines exactly one of MB200_USER_DIAGONAL_METRIC, MB200_USER_SCALAR_METRIC and
-// MB200_USER_DENSE_METRIC and puts MB200_USER_METRIC_FUNCTIONS after the user sources: that binds
-// the pair to the policies, so a missing function is reported at the end of the user's own source.
+// The Cholesky-factored metric runs on the triangular-factored policy CholeskyFactoredMetric (K10):
+// one 256-thread CTA (MB200_RM_CHOL_THREADS) per chain, with the same CtaChain view and the same
+// rules as the dense metric: both functions are called by the whole CTA, each call between two
+// __syncthreads(), and the target keeps its warp contract through warp 0.  L and V are [dim x
+// (dim + 1)] matrices in shared memory up to D = 112 and in a per-CTA global workspace beyond;
+// q and out are in shared memory.  The policy forms V itself, lower triangle only: diag(2 / L_ii)
+// for the gradient of log|M| and tril(-2 (M^-1 p)(L^-1 p)^T) for that of the quadratic form, and
+// calls vjp_metric_chol once for each.  As in the reference (TriangularFactoredPositiveDefinite-
+// Matrix): a non-finite entry of the lower triangle is a LinAlgError (the policy checks the
+// lower triangle after every fill), a ConvergenceError inside a fixed-point solve; a negative
+// diagonal entry is legal; a zero one fails only where L is solved with.  dim <= 1016, where the
+// per-chain vectors alone fill the shared memory.
+//
+// The host defines exactly one of MB200_USER_DIAGONAL_METRIC, MB200_USER_SCALAR_METRIC,
+// MB200_USER_DENSE_METRIC and MB200_USER_CHOLESKY_METRIC and puts MB200_USER_METRIC_FUNCTIONS
+// after the user sources: that binds the pair to the policies, so a missing function is reported
+// at the end of the user's own source.
 #pragma once
 #include "user_target.cuh"
 #include "riemannian.cuh"
 
 #if defined(MB200_USER_DIAGONAL_METRIC) + defined(MB200_USER_SCALAR_METRIC) + \
-        defined(MB200_USER_DENSE_METRIC) != 1
-#error "define exactly one of MB200_USER_DIAGONAL_METRIC, MB200_USER_SCALAR_METRIC and MB200_USER_DENSE_METRIC"
+        defined(MB200_USER_DENSE_METRIC) + defined(MB200_USER_CHOLESKY_METRIC) != 1
+#error "define exactly one of MB200_USER_DIAGONAL_METRIC, MB200_USER_SCALAR_METRIC, MB200_USER_DENSE_METRIC and MB200_USER_CHOLESKY_METRIC"
 #endif
 
 #ifdef MB200_USER_DENSE_METRIC
@@ -156,8 +177,7 @@ using UserDiagonalMetric = DiagonalMetric<Target, UserDiagModel<>>;
 template <class Target>
 using UserScalarMetric = ScalarMetric<Target, UserScalarModel<>>;
 
-#ifdef MB200_USER_DENSE_METRIC
-// What a dense metric function sees of one chain: the whole CTA
+// What a dense or Cholesky-factored metric function sees of one chain: the whole CTA
 struct CtaChain {
   int dim;
   int lane;                         // 0 .. n_lanes - 1: the thread of the CTA
@@ -171,9 +191,10 @@ struct CtaChain {
   __device__ __forceinline__ double sum(double x) const { return block_sum(blk, x); }
 };
 
-// The target's warp contract on the dense policy's 256-thread CTA: warp 0 calls the user
-// functions, the other warps wait at the barrier; the value of l reaches every thread through
-// shared memory (the reduction scratch's slot 32, which block_sum / block_nanmax never use)
+// The target's warp contract on a 256-thread CTA (the dense and Cholesky-factored policies):
+// warp 0 calls the user functions, the other warps wait at the barrier; the value of l reaches
+// every thread through shared memory (the reduction scratch's slot 32, which block_sum /
+// block_nanmax / block_prefix_suffix never use)
 struct UserRTargetCta : UserRTarget {
   __device__ UserRTargetCta(const ModelArgs& m, int d) : UserRTarget(m, d) {}
   __device__ double nld(const Blk& k, const double* q) const {
@@ -192,6 +213,57 @@ struct UserRTargetCta : UserRTarget {
   }
 };
 
+// The CTA-wide metric's view of a chain: rmetric_params and rmetric_aux, read from the kernel's
+// ModelArgs parameter at each call rather than held in registers across the integrator
+struct UserCtaMetricArgs {
+  const ModelArgs& m;
+  int dim;
+  __device__ UserCtaMetricArgs(const ModelArgs& mm, int d) : m(mm), dim(d) {}
+  __device__ __forceinline__ CtaChain chain(const Blk& k, const double* q) const {
+    CtaChain c;
+    c.dim = dim;
+    c.lane = k.tid;
+    c.n_lanes = k.nthr;
+    c.q = q;
+#pragma unroll
+    for (int i = 0; i < MB200_MAX_PARAMS; ++i) c.params[i] = m.mp[i];
+    c.aux = m.maux;
+    c.blk = k;
+    return c;
+  }
+};
+
+// CholeskyFactoredMetric's model interface over metric_chol / vjp_metric_chol: fill, then the
+// policy's own finiteness check of the lower triangle (the user function returns nothing), and
+// the VJP of a lower-triangular V (DENSE_VJP: the policy forms V in w.M2)
+template <class F = UserMetricFunctions>
+struct UserCholModel : UserCtaMetricArgs {
+  static constexpr bool DENSE_VJP = true;
+  __device__ UserCholModel(const ModelArgs& m, int d) : UserCtaMetricArgs(m, d) {}
+  // true iff every entry of the lower triangle is finite
+  __device__ bool fill(const Blk& k, const double* q, double* L, int ld) const {
+    __syncthreads();
+    F::chol(chain(k, q), L, ld);
+    __syncthreads();
+    bool bad = false;
+    for (int i = k.warp; i < dim; i += k.nwarp)
+      for (int j = k.lane; j <= i; j += 32)
+        if (!isfinite(L[i * ld + j])) bad = true;
+    return !bad;
+  }
+  __device__ void vjp_tril(const Blk& k, const double* q, const double* V, int ld,
+                           double* out) const {
+    __syncthreads();
+    F::vjp(chain(k, q), V, ld, out);
+    __syncthreads();
+  }
+};
+
+template <class Target>
+using UserCholeskyMetric = CholeskyFactoredMetric<Target, UserCholModel<>>;
+static_assert(MB200_RM_CHOL_THREADS == 256, "the Cholesky user contract is per 256-thread CTA");
+
+#ifdef MB200_USER_DENSE_METRIC
 // GlobalDenseMetricT's model interface over metric_dense / vjp_metric_dense: fill and the dense
 // VJP, no entry and no rank-one VJP (the policy forms V = -w w^T for the generic route)
 template <class F = UserMetricFunctions>
@@ -243,6 +315,15 @@ static_assert(user_policy_traits_match<DiagonalMetric<UserRTarget, QuadraticDiag
                   user_policy_traits_match<ScalarMetric<UserRTarget, QuadraticScalarModel>>(),
               "host launch traits");
 
+template <class P>
+constexpr bool user_chol_traits_match() {
+  using H = UserRCholPolicyTraits<UserRTargetCta>;
+  return P::SOFTABS == H::SOFTABS && rm_compact_policy<P>::value == H::COMPACT &&
+         P::N_MATS == H::N_MATS && rm_workspace_mats<P>::value == H::WORKSPACE_MATS &&
+         P::MIN_BLOCKS == H::MIN_BLOCKS && P::THREADS == H::THREADS;
+}
+static_assert(user_chol_traits_match<UserCholeskyMetric<UserRTargetCta>>(), "host launch traits");
+
 }  // namespace mb200
 
 #ifdef MB200_USER_DIAGONAL_METRIC
@@ -265,6 +346,17 @@ static_assert(user_policy_traits_match<DiagonalMetric<UserRTarget, QuadraticDiag
     static __device__ __forceinline__ void vjp(const mb200::CtaChain& c, const double* V,       \
                                                int ld, double* out) {                           \
       vjp_metric_dense(c, V, ld, out);                                                          \
+    }                                                                                           \
+  };
+#elif defined(MB200_USER_CHOLESKY_METRIC)
+#define MB200_USER_METRIC_FUNCTIONS                                                             \
+  struct mb200::UserMetricFunctions {                                                           \
+    static __device__ __forceinline__ void chol(const mb200::CtaChain& c, double* L, int ld) {  \
+      metric_chol(c, L, ld);                                                                    \
+    }                                                                                           \
+    static __device__ __forceinline__ void vjp(const mb200::CtaChain& c, const double* V,       \
+                                               int ld, double* out) {                           \
+      vjp_metric_chol(c, V, ld, out);                                                           \
     }                                                                                           \
   };
 #else

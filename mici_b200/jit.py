@@ -15,7 +15,7 @@ carries the constrained leapfrog and projection kernels (``csrc/constrained.cuh`
 constraint count and KP; its cache key covers both and whether the source defines
 ``mhp_constr``.
 
-A user target paired with a user diagonal, scalar or dense metric (contract:
+A user target paired with a user diagonal, scalar, dense or Cholesky-factored metric (contract:
 ``csrc/user_riemannian.cuh``) compiles into an image of its own: the implicit-integrator, velocity
 and momentum-refresh kernels of ``csrc/riemannian.cuh`` for that (target, metric) pair -- on the
 global-workspace dense policy of ``csrc/dense_global.cuh`` for a dense metric -- keyed on both
@@ -31,7 +31,12 @@ import os
 import threading
 
 from .errors import Error, TargetCompileError
-from .targets import RMETRIC_USER_DENSE, RMETRIC_USER_DIAGONAL, RMETRIC_USER_SCALAR
+from .targets import (
+    RMETRIC_USER_CHOLESKY,
+    RMETRIC_USER_DENSE,
+    RMETRIC_USER_DIAGONAL,
+    RMETRIC_USER_SCALAR,
+)
 
 _PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_PKG, "csrc")
@@ -61,16 +66,20 @@ def constrained_name_expressions(kp):
 
 # The kernels of a Riemannian image, in the kernel-table order of mb200_user_riemannian_load:
 # implicit leapfrog / midpoint, velocity, momentum refresh
-RIEMANNIAN_KINDS = ("diagonal", "scalar", "dense")
+RIEMANNIAN_KINDS = ("diagonal", "scalar", "dense", "cholesky")
 # the rmetric_id a Riemannian image serves, by metric kind
 RIEMANNIAN_RMETRIC_IDS = {"diagonal": RMETRIC_USER_DIAGONAL, "scalar": RMETRIC_USER_SCALAR,
-                          "dense": RMETRIC_USER_DENSE}
+                          "dense": RMETRIC_USER_DENSE, "cholesky": RMETRIC_USER_CHOLESKY}
+# the metric kinds whose policy runs a 256-thread CTA per chain: the metric functions see the
+# whole CTA (mb200::CtaChain), the target's warp functions run on warp 0
+CTA_KINDS = ("dense", "cholesky")
 
 
 def riemannian_name_expressions(kind):
     m = "mb200::User%sMetric" % kind.capitalize()
-    # the dense policy's 256-thread CTA calls the target's warp functions from warp 0 only
-    t = "mb200::UserRTargetCta" if kind == "dense" else "mb200::UserRTarget"
+    # the 256-thread CTA of the dense and Cholesky-factored policies calls the target's warp
+    # functions from warp 0 only
+    t = "mb200::UserRTargetCta" if kind in CTA_KINDS else "mb200::UserRTarget"
     return tuple(f"&mb200::{k}<{t}, {m}>"
                  for k in ("implicit_leapfrog_kernel", "riemannian_velocity_kernel",
                            "riemannian_sample_momentum_kernel"))
@@ -252,7 +261,7 @@ def compile_target(source, name="user_target", *, n_constr=0, kp=0, mhp_constr=F
     """Compile a user target; returns ``(key, cubin, lowered kernel names)``, from the process
     cache when the same source was compiled before.  ``n_constr >= 1``: a constrained target,
     whose image also carries the constrained kernels at ``kp``.  ``metric = (kind, source,
-    name)``, kind ``"diagonal"``, ``"scalar"`` or ``"dense"``: the Riemannian image of the target
+    name)``, kind ``"diagonal"``, ``"scalar"``, ``"dense"`` or ``"cholesky"``: the Riemannian image of the target
     with that user metric.  Raises ``TargetCompileError`` with the NVRTC log on failure."""
     constraint = _constraint(n_constr, kp, mhp_constr)
     metric = _metric(metric)

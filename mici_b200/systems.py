@@ -30,6 +30,7 @@ from .errors import LinAlgError
 from .solvers import solve_projection_onto_manifold_newton
 from .targets import (
     RMETRIC_SOFTABS,
+    CudaCholeskyMetric,
     CudaDenseMetric,
     CudaDiagonalMetric,
     CudaRiemannianPair,
@@ -847,17 +848,29 @@ class CholeskyFactoredRiemannianMetricSystem(RiemannianMetricSystem):
     is built -- status 3 (``LinAlgError``) outside a fixed-point solve, ``ConvergenceError``
     inside one.  A negative diagonal entry is legal.  A zero diagonal entry fails only where the
     metric is solved with: ``dh_dmom`` raises ``LinAlgError``, ``h`` is NaN, ``sample_momentum``
-    succeeds, and an integrator step ends in ``ConvergenceError`` (DESIGN.md section 1)."""
+    succeeds, and an integrator step ends in ``ConvergenceError`` (DESIGN.md section 1).
+
+    ``metric_chol_func`` may also be a user-written ``mici_b200.targets.CudaCholeskyMetric`` with
+    an unconstrained ``CudaTarget`` (``dim <= 1016``), with the same failure rules; its factor and
+    the matrix its VJP takes stay in shared memory up to D = 112."""
+
+    # the largest dimension whose per-chain vectors fit in shared memory beside the workspace
+    MAX_USER_DIM = 1016
 
     def __init__(self, neg_log_dens, metric_chol_func, *, vjp_metric_chol_func=None,
                  grad_neg_log_dens=None, backend=None):
+        self._accept_user_metric(neg_log_dens, metric_chol_func, CudaCholeskyMetric)
         super().__init__(neg_log_dens, grad_neg_log_dens=grad_neg_log_dens, backend=backend)
-        if not isinstance(metric_chol_func, QuadraticCholeskyMetric):
+        if not isinstance(metric_chol_func, (QuadraticCholeskyMetric, CudaCholeskyMetric)):
             raise TypeError("`metric_chol_func` must be a registered metric model "
-                            "(QuadraticCholeskyMetric).")
+                            "(QuadraticCholeskyMetric) or a CudaCholeskyMetric.")
         if vjp_metric_chol_func is not None:
             raise ValueError("The metric VJP is fused into the kernels.")
-        if metric_chol_func.dim != neg_log_dens.dim:
+        if isinstance(metric_chol_func, CudaCholeskyMetric):
+            if neg_log_dens.dim > self.MAX_USER_DIM:
+                raise ValueError(f"A CudaCholeskyMetric needs dim <= {self.MAX_USER_DIM}, "
+                                 f"got {neg_log_dens.dim}.")
+        elif metric_chol_func.dim != neg_log_dens.dim:
             raise ValueError(f"The base factor is {metric_chol_func.dim} x {metric_chol_func.dim}; "
                              f"the target has dimension {neg_log_dens.dim}.")
         self.metric_model = metric_chol_func

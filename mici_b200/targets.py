@@ -32,6 +32,7 @@ RMETRIC_CHOL_QUADRATIC = 6
 RMETRIC_USER_DIAGONAL = 32  # MB200_RMETRIC_USER_DIAGONAL: CudaDiagonalMetric
 RMETRIC_USER_SCALAR = 33  # MB200_RMETRIC_USER_SCALAR: CudaScalarMetric
 RMETRIC_USER_DENSE = 34  # MB200_RMETRIC_USER_DENSE: CudaDenseMetric
+RMETRIC_USER_CHOLESKY = 35  # MB200_RMETRIC_USER_CHOLESKY: CudaCholeskyMetric
 
 
 class Target:
@@ -238,7 +239,8 @@ class CudaTarget(Target):
 
 
 class _CudaMetric:
-    """A user-written diagonal, scalar or dense metric (contract: ``mici_b200/csrc/user_riemannian.cuh``):
+    """A user-written diagonal, scalar, dense or Cholesky-factored metric (contract:
+    ``mici_b200/csrc/user_riemannian.cuh``):
     CUDA C++ source, at most 8 ``params`` (``c.params`` inside the metric functions) and an
     optional ``aux`` array (``c.aux``).  It runs with a ``CudaTarget`` only, compiled with it into
     one image; like the target it holds only source, params and aux."""
@@ -315,6 +317,29 @@ class CudaDenseMetric(_CudaMetric):
 
     kind = "dense"
     rmetric_id = RMETRIC_USER_DENSE
+
+
+class CudaCholeskyMetric(_CudaMetric):
+    """A user-written metric M(q) = L(q) L(q)^T given by its lower-triangular factor, for
+    ``CholeskyFactoredRiemannianMetricSystem``: CUDA C++ source defining
+
+        __device__ void metric_chol(const mb200::CtaChain& c, double* L, int ld);
+        __device__ void vjp_metric_chol(const mb200::CtaChain& c, const double* V, int ld,
+                                        double* out);
+
+    with ``L[i * ld + j] = L_ij(q)`` for ``0 <= j <= i < dim`` (the upper triangle is never read)
+    and ``out[k] = sum_{j <= i} V[i * ld + j] dL_ij/dq_k``, every ``out[k], k < dim`` written, for
+    a lower-triangular ``V`` whose entries above the diagonal must not be read.  These are the
+    reference's ``metric_chol_func`` and ``vjp_metric_chol_func(q)(V)``.  Both functions are
+    called by the whole 256-thread CTA of the chain (``c.lane`` in ``[0, c.n_lanes)``,
+    ``c.sum()`` a CTA all-reduce), as for ``CudaDenseMetric``; the target keeps its warp contract.
+    No factorisation: O(D^2) per metric.  A non-finite entry of the lower triangle is a
+    ``LinAlgError`` outside a fixed-point solve and a ``ConvergenceError`` inside one; a negative
+    diagonal entry is legal; a zero one fails only where ``L`` is solved with.  ``dim <= 1016``.
+    Contract: ``mici_b200/csrc/user_riemannian.cuh``."""
+
+    kind = "cholesky"
+    rmetric_id = RMETRIC_USER_CHOLESKY
 
 
 class CudaRiemannianPair:
