@@ -17,7 +17,7 @@ int64_t dense_global_workspace_bytes(int64_t n_chains, int dim) {
 }
 
 bool dense_global_supported(int dim) {
-  return rm_smem_doubles(dim, RM_NMATS_GLOBAL) * sizeof(double) <= 227 * 1024;
+  return rm_smem_bytes(dg_layout(dim)) <= RM_SMEM_BYTES;
 }
 
 // The kernels this plan starts: a registry instantiation, or a kernel of a loaded user image (a
@@ -26,7 +26,8 @@ using DgImplicitKernel = decltype(&implicit_leapfrog_kernel<QuadraticRTarget, Gl
 using DgVectorKernel = decltype(&riemannian_velocity_kernel<QuadraticRTarget, GlobalDenseRank1>);
 
 static int dg_launch_implicit(DgImplicitKernel kern, const ImplicitArgs& a) {
-  const size_t smem = rm_smem_doubles(a.dim, RM_NMATS_GLOBAL) * sizeof(double);
+  const RmLayout layout = dg_layout(a.dim);
+  const size_t smem = rm_smem_bytes(layout);
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
   const int blocks = dg_blocks(a.n);
@@ -37,7 +38,7 @@ static int dg_launch_implicit(DgImplicitKernel kern, const ImplicitArgs& a) {
   m.ws_stride = dg_workspace_doubles(a.dim);
   rm_start(kern, (unsigned)blocks, DG_THREADS, smem, a.st, a.q_in, a.p_in, a.q_out, a.p_out, a.dir,
            a.n, a.dim, a.eps, a.n_steps, m, a.fp_tol, a.fp_div, a.fp_max, a.rev_tol, a.h_out,
-           a.status, a.n_done, a.fp_iters, RM_NMATS_GLOBAL, 0, a.fp_solver);
+           a.status, a.n_done, a.fp_iters, layout, 0, a.fp_solver);
   return check_launch("implicit_leapfrog_kernel (global dense metric)");
 }
 
@@ -52,7 +53,8 @@ int dense_global_implicit_image(const ImplicitArgs& a, const void* kern) {
 }
 
 static int dg_launch_vec(DgVectorKernel kern, const VectorArgs& a) {
-  const size_t smem = rm_smem_doubles(a.dim, RM_NMATS_GLOBAL) * sizeof(double);
+  const RmLayout layout = dg_layout(a.dim);
+  const size_t smem = rm_smem_bytes(layout);
   const int blocks = dg_blocks(a.n);
   DgScratch scratch(nullptr, 0, (size_t)dense_global_workspace_bytes(a.n, a.dim), a.st);
   if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "dense metric workspace allocation failed");
@@ -62,7 +64,7 @@ static int dg_launch_vec(DgVectorKernel kern, const VectorArgs& a) {
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
   rm_start(kern, (unsigned)blocks, DG_THREADS, smem, a.st, a.q, a.v, a.out, a.n, a.dim, m,
-           a.status, RM_NMATS_GLOBAL);
+           a.status, layout);
   return check_launch("riemannian vector kernel (global dense metric)");
 }
 
@@ -99,7 +101,7 @@ int mb200_selftest_dense_factor(const double* matrices, const double* rhs, int64
     return fail(MB200_ERR_UNSUPPORTED, "dim %d: panel buffers exceed shared memory", dim);
   const DeviceScope device_scope(matrices);
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t smem = rm_smem_doubles(dim, RM_NMATS_GLOBAL) * sizeof(double);
+  const size_t smem = rm_smem_bytes(dg_layout(dim));
   cudaError_t e = cudaFuncSetAttribute(dense_global_selftest_kernel,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));

@@ -9,40 +9,40 @@ namespace mb200 {
 enum class RmOp { Leapfrog, Midpoint, SampleMomentum, Velocity };
 
 // Launch plan of the three Riemannian kernels outside the global-workspace dense policy: the
-// shared-memory layout (n_mats), the per-CTA global workspace of the policies whose matrices do
-// not fit in shared memory, and the grid.  `launch(blocks, smem, margs, n_mats)` starts `kern`.
+// chain's layout, the per-CTA global workspace of the policies whose matrices do not fit in
+// shared memory, and the grid.  `launch(blocks, smem, margs, layout)` starts `kern`.
 template <class Target, template <class> class MetricT, class Kernel, class Launch>
 static int rm_launch(Kernel kern, const char* name, RmOp op, int64_t n, int dim,
                      const ModelArgs& m, cudaStream_t st, const Launch& launch) {
   using Metric = MetricT<Target>;
-  constexpr bool compact = rm_compact_policy<Metric>::value;
-  constexpr int ws_mats = rm_workspace_mats<Metric>::value;
+  constexpr bool compact = Metric::PLACE == RM_COMPACT;
   const bool implicit = op == RmOp::Leapfrog || op == RmOp::Midpoint;
-  int n_mats = Metric::N_MATS;
+  RmLayout layout{dim, Metric::PLACE, Metric::N_MATS, 0, op == RmOp::Midpoint};
   // SoftAbs integrators: a third matrix enables warm-started eigensolves; use it when two CTAs
   // still fit (DENSE_MTP targets always: the third holds Z = A U)
-  if (Metric::SOFTABS && implicit &&
-      (rm_smem_doubles(dim, 3) * sizeof(double) <= 113 * 1024 || Target::DENSE_MTP))
-    n_mats = 3;
-  size_t smem = (compact ? rm_compact_doubles(dim, op == RmOp::Midpoint)
-                         : rm_smem_doubles(dim, n_mats)) * sizeof(double);
-  bool in_ws = false;
-  if (smem > 227 * 1024) {
+  if (Metric::SOFTABS && implicit) {
+    RmLayout three = layout;
+    three.smem_mats = 3;
+    if (rm_smem_bytes(three) <= 113 * 1024 || Target::DENSE_MTP) layout = three;
+  }
+  size_t smem = rm_smem_bytes(layout);
+  if (smem > RM_SMEM_BYTES) {
     if (compact && implicit)
       return fail(MB200_ERR_UNSUPPORTED,
                   "dim %d: per-chain vectors (%zu bytes) exceed shared memory", dim, smem);
     // SoftAbs and Cholesky-factored metrics beyond shared memory: the same kernels with the
     // matrices in a per-CTA global workspace (L2-resident operands: slower, but the reference
     // has no dimension limit)
-    if (ws_mats == 0)
+    if (Metric::WORKSPACE_MATS == 0)
       return implicit ? fail(MB200_ERR_UNSUPPORTED,
                              "dim %d: per-chain metric (%zu bytes) exceeds shared memory", dim, smem)
                       : fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
-    n_mats = RM_NMATS_IN_WORKSPACE + ws_mats;
-    smem = rm_smem_doubles(dim, n_mats) * sizeof(double);
-    in_ws = true;
-    if (smem > 227 * 1024) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
+    layout.smem_mats = 0;
+    layout.ws_mats = Metric::WORKSPACE_MATS;
+    smem = rm_smem_bytes(layout);
+    if (smem > RM_SMEM_BYTES) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large", dim);
   }
+  const bool in_ws = layout.ws_mats > 0;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));
   // the integrators and the small CTAs of the compact policies: as many CTAs as fit (at most two
@@ -57,21 +57,25 @@ static int rm_launch(Kernel kern, const char* name, RmOp op, int64_t n, int dim,
   int64_t blocks = (int64_t)num_sms() * per_sm;
   if (blocks > n) blocks = n;
   ModelArgs margs = m;
-  const size_t per_cta = ws_mats * ((((size_t)dim * (dim + 1)) + 1) & ~(size_t)1);
+  const size_t per_cta = layout.ws_mats * layout.ws_mat_doubles();
   DgScratch scratch(nullptr, 0, in_ws ? per_cta * blocks * sizeof(double) : 0, st);
   if (in_ws) {
     if (scratch.ptr == nullptr) return fail(MB200_ERR_CUDA, "metric workspace allocation failed");
     margs.workspace = scratch.ptr;
     margs.ws_stride = per_cta;
   }
-  launch((unsigned)blocks, smem, margs, n_mats);
+  launch((unsigned)blocks, smem, margs, layout);
   return check_launch(name);
 }
 
+// a user image's Cholesky-factored policy as the host plans it
+template <class Target>
+using UserCholeskyPlan = CholeskyFactoredMetric<Target, UserCholModelTraits>;
+
 // Launch functors of the operations: `run<Target, MetricT>()` starts the operation's kernel for
 // that pair, `global(hadamard)` its global-workspace dense form (api_dense.cu), `image<Traits>()`
-// the kernel of the loaded user image `user` (user_riemannian.cuh), planned from the traits the
-// image's policy shares with the host (UserRPolicyTraits, UserRCholPolicyTraits)
+// the kernel of the loaded user image `user` (user_riemannian.cuh), planned as the registry
+// policy `Traits` over UserRTargetTraits, whose launch constants the image's policy shares
 using ImplicitKernel = decltype(&implicit_leapfrog_kernel<StdGaussianRTarget, QuadraticDiagonalMetric>);
 using VectorKernel = decltype(&riemannian_velocity_kernel<StdGaussianRTarget, QuadraticDiagonalMetric>);
 
@@ -92,10 +96,10 @@ struct ImplicitLaunch {
   int launch(ImplicitKernel kern) const {
     return rm_launch<Target, MetricT>(
         kern, "implicit_leapfrog_kernel", OP, a.n, a.dim, a.m, a.st,
-        [&](unsigned blocks, size_t smem, const ModelArgs& margs, int n_mats) {
+        [&](unsigned blocks, size_t smem, const ModelArgs& margs, const RmLayout& layout) {
           rm_start(kern, blocks, MetricT<Target>::THREADS, smem, a.st, a.q_in, a.p_in, a.q_out,
                    a.p_out, a.dir, a.n, a.dim, a.eps, a.n_steps, margs, a.fp_tol, a.fp_div,
-                   a.fp_max, a.rev_tol, a.h_out, a.status, a.n_done, a.fp_iters, n_mats,
+                   a.fp_max, a.rev_tol, a.h_out, a.status, a.n_done, a.fp_iters, layout,
                    (int)(OP == RmOp::Midpoint), a.fp_solver);
         });
   }
@@ -122,9 +126,10 @@ struct VectorLaunch {
   int launch(VectorKernel kern) const {
     return rm_launch<Target, MetricT>(
         kern, velocity ? "riemannian_velocity_kernel" : "riemannian_sample_momentum_kernel", OP,
-        a.n, a.dim, a.m, a.st, [&](unsigned blocks, size_t smem, const ModelArgs& margs, int n_mats) {
+        a.n, a.dim, a.m, a.st,
+        [&](unsigned blocks, size_t smem, const ModelArgs& margs, const RmLayout& layout) {
           rm_start(kern, blocks, MetricT<Target>::THREADS, smem, a.st, a.q, a.v, a.out, a.n, a.dim,
-                   margs, a.status, n_mats);
+                   margs, a.status, layout);
         });
   }
   int global(bool hadamard) const { return dense_global_vector(a, velocity, hadamard); }
@@ -170,9 +175,10 @@ static int run_on_target(int target_id, const L& l, const char* metric) {
 // checks whatever the operation), picks the metric policy and the target, and hands them to `l`.
 // An operation's exclusions sit next to the route they restrict.  A loaded user image (l.user,
 // the *_user entry points) serves a user target with the image's own user metric, planned from
-// the host traits of its policy: the compact ones (diagonal, scalar), the triangular-factored one
-// (MB200_RMETRIC_USER_CHOLESKY: 256-thread CTAs, the factor and V per chain), or, for a dense
-// one (MB200_RMETRIC_USER_DENSE), the global-workspace launch plan with its limits.
+// the registry policy it runs over user models: the compact ones (diagonal, scalar), the
+// triangular-factored one (MB200_RMETRIC_USER_CHOLESKY: 256-thread CTAs, the factor and V per
+// chain), or, for a dense one (MB200_RMETRIC_USER_DENSE), the global-workspace launch plan with its
+// limits.
 template <class L>
 static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
   constexpr RmOp op = L::op;
@@ -184,9 +190,11 @@ static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
       return fail(MB200_ERR_INVALID_ARG, "rmetric_id %d does not match the user image's (%d)",
                   m.rmetric_id, l.user->rmetric_id);
     if (l.user->rmetric_id == MB200_RMETRIC_USER_CHOLESKY)
-      return l.template image<UserRCholPolicyTraits>();
+      return l.template image<UserCholeskyPlan>();
+    if (l.user->rmetric_id == MB200_RMETRIC_USER_SCALAR)
+      return l.template image<QuadraticScalarMetric>();
     if (l.user->rmetric_id != MB200_RMETRIC_USER_DENSE)
-      return l.template image<UserRPolicyTraits>();
+      return l.template image<QuadraticDiagonalMetric>();
     if (op == RmOp::Midpoint)
       return fail(MB200_ERR_UNSUPPORTED,
                   "implicit midpoint is not available for the global-workspace dense metric");
@@ -195,7 +203,7 @@ static int rm_dispatch(const ModelArgs& m, int dim, const L& l) {
     return l.image_global();
   }
   // one per-chain D x D matrix (the rank-1 metric's Cholesky factor) fits in shared memory
-  const bool fits = rm_smem_doubles(dim, 1) * sizeof(double) <= 227 * 1024;
+  const bool fits = rm_smem_bytes(RmLayout{dim, RM_MATRICES, 1, 0, true}) <= RM_SMEM_BYTES;
 
   // Global-workspace dense policy: every Hadamard metric, and the rank-1 metric whose factor does
   // not fit in shared memory on the quadratic target, unless the Sherman-Morrison form is forced
@@ -433,8 +441,9 @@ int mb200_selftest_eigh(const double* matrices, int64_t n_matrices, int32_t dim,
     return fail(MB200_ERR_INVALID_ARG, "bad arguments");
   if (n_matrices == 0) return 0;
   const DeviceScope device_scope(matrices);
-  const size_t smem = rm_smem_doubles(dim, 3) * sizeof(double);
-  if (smem > 227 * 1024) return fail(MB200_ERR_UNSUPPORTED, "dim %d too large for the self-test", dim);
+  const size_t smem = rm_smem_bytes(eigh_selftest_layout(dim));
+  if (smem > RM_SMEM_BYTES)
+    return fail(MB200_ERR_UNSUPPORTED, "dim %d too large for the self-test", dim);
   cudaError_t e = cudaFuncSetAttribute(eigh_selftest_kernel,
                                        cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) return fail(MB200_ERR_CUDA, "smem attr: %s", cudaGetErrorString(e));

@@ -56,6 +56,11 @@ __host__ __device__ inline size_t dg_workspace_doubles(int dim) {
   return 3 * np * np + (np / DG_NB) * DG_NB * DG_NB;
 }
 
+// a chain's layout under this policy
+__host__ __device__ inline RmLayout dg_layout(int dim) {
+  return RmLayout{dim, RM_DENSE_GLOBAL, 0, 0, false};
+}
+
 __device__ inline void dg_attach(DgWork& g, const RmWork& w, const ModelArgs& m) {
   g.n = w.dim;
   g.np = dg_padded_dim(w.dim);
@@ -627,7 +632,7 @@ struct dg_model_rank1<M, decltype(void(&M::vjp_rank1))> {
 template <class Target, class Model>
 struct GlobalDenseMetricT {
   static constexpr bool SOFTABS = false;
-  static constexpr int N_MATS = RM_NMATS_GLOBAL;
+  static constexpr RmPlace PLACE = RM_DENSE_GLOBAL;
   static constexpr int MIN_BLOCKS = 1;  // ~200 KB of shared memory per CTA: one CTA per SM
   static constexpr int THREADS = DG_THREADS;
   const Target& t;
@@ -769,12 +774,9 @@ static __global__ void __launch_bounds__(DG_THREADS)
                                  double* __restrict__ chol_out, double* __restrict__ inv_out,
                                  double* __restrict__ sol_out, double* __restrict__ logdet_out,
                                  int32_t* __restrict__ status) {
-  extern __shared__ double smem[];
   Blk k;
-  k.tid = threadIdx.x, k.nthr = blockDim.x, k.lane = threadIdx.x & 31;
-  k.warp = threadIdx.x >> 5, k.nwarp = blockDim.x >> 5;
   RmWork w;
-  rm_carve(w, smem, dim, RM_NMATS_GLOBAL, k);
+  rm_begin<false>(dg_layout(dim), margs, k, w);
   DgWork g;
   dg_attach(g, w, margs);
   const int n = dim, np = g.np;

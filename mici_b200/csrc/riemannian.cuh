@@ -385,39 +385,83 @@ __host__ __device__ inline size_t dg_smem_doubles(int dim) {
   const int np = dg_padded_dim(dim);
   return (size_t)(np > 32 ? np - 32 : 32) * 36 + 2 * 32 * 36;
 }
-constexpr int RM_NMATS_GLOBAL = -1;  // n_mats code: compact vector set + dg_smem_doubles()
-// n_mats code RM_NMATS_IN_WORKSPACE + k: the k per-chain D x D matrices of the shared-memory
-// policies (SoftAbs: eigenvectors, work / divided-difference matrix, warm-start matrix) live in
-// the per-CTA GLOBAL workspace instead (dimensions whose matrices exceed 227 KB: SoftAbs at
-// D > ~100, the Cholesky-factored metric's factor at D > ~150); the algorithms are unchanged,
-// the operands are simply L2-resident
-constexpr int RM_NMATS_IN_WORKSPACE = 100;
+// opt-in dynamic shared memory of one CTA on sm_90 (228 KB per SM, 1 KB of it reserved per CTA)
+constexpr size_t RM_SMEM_BYTES = 227 * 1024;
 
-// n_mats: per-chain D x D matrices kept in shared memory (SoftAbs 2, or 3 with warm-started
-// eigensolves; dense Cholesky 1; Sherman-Morrison 0)
-__host__ __device__ inline size_t rm_smem_doubles(int dim, int n_mats) {
-  const int ld = dim + 1;
-  const int dpad = (dim + 1) & ~1;
-  if (n_mats == RM_NMATS_GLOBAL)  // q p qs ps x0 x1 x2 base v1 v2 v3 ev + scratch + panel buffers
-    return (size_t)12 * dpad + 40 + dg_smem_doubles(dim);
-  if (n_mats >= RM_NMATS_IN_WORKSPACE) n_mats = 0;  // matrices in the global workspace
-  size_t n = (size_t)dim * ld * n_mats;
-  n += (size_t)16 * dpad;      // vectors (Vn counts double: NEED <= 2)
-  n += (size_t)dpad;           // second half of Vn
-  n += (size_t)10 * dpad;      // z0, z1, z2, zb, zp (2 * dpad each)
-  n += 2 * (size_t)(dpad / 2 + 2);  // rc, rs
-  n += (size_t)(dpad / 2 + 2);      // top, bot (ints, 2 per double)
-  n += 40;                     // reduction scratch
-  return n;
-}
+// Where a chain's buffers live.  Every metric policy declares its PLACE; those that rm_launch
+// plans also declare the per-chain D x D matrices they keep in shared memory (N_MATS) and how many
+// of them move to the per-CTA global workspace when those do not fit (WORKSPACE_MATS, 0: no such
+// route).
+enum RmPlace : int {
+  // the O(D) policies (diagonal and scalar metrics): the integrator's vectors plus ev (policy
+  // scratch), lam (d(q)) and sa (1 / d(q)), and the implicit-midpoint vectors only for implicit
+  // midpoint; no matrices, no eigensolver or Cholesky buffers: at D = 128 a chain needs 14.6 KB
+  // (leapfrog), so that many chains share an SM
+  RM_COMPACT,
+  // the matrix policies: every vector, and the matrices in shared memory or, beyond it (SoftAbs
+  // at D > ~100, the Cholesky-factored metric's factor at D > ~150), in the per-CTA global
+  // workspace: the algorithms are unchanged, the operands are simply L2-resident
+  RM_MATRICES,
+  // the global-workspace dense policy (dense_global.cuh): the integrator's vectors and ev, then
+  // its panel buffers (dg_smem_doubles) from `extra`
+  RM_DENSE_GLOBAL,
+};
 
-__device__ inline void rm_carve(RmWork& w, double* s, int dim, int n_mats, Blk& blk,
-                                double* gmats = nullptr) {
+// The layout of one chain's buffers: planned on the host (rm_launch, the dense-global launchers)
+// and passed to the kernels
+struct RmLayout {
+  int dim;
+  RmPlace place;
+  int smem_mats;  // RM_MATRICES: per-chain D x (D + 1) matrices in shared memory
+  int ws_mats;    // ... or in the per-CTA global workspace (then smem_mats == 0)
+  bool zvecs;     // RM_COMPACT: the implicit-midpoint vectors too (RM_MATRICES: always)
+  // doubles from one workspace matrix to the next (each starts 16-byte aligned); a CTA's
+  // workspace is ws_mats of them
+  __host__ __device__ size_t ws_mat_doubles() const {
+    return ((size_t)dim * (dim + 1) + 1) & ~(size_t)1;
+  }
+};
+
+// Carves the buffers of layout `l` from shared memory `s` and this CTA's workspace `gmats`: every
+// pointer of `w` (those the layout lacks are NULL), the reduction scratch blk.red [40 doubles],
+// `extra` (what follows it) and *tscratch, the [dim] scratch of DENSE_MTP targets.  Returns the
+// doubles of shared memory the layout takes; the host sizes a launch by running it from a null
+// base (rm_smem_bytes), so the size and the pointers cannot disagree.  Vectors are dpad apart:
+//   RM_COMPACT       q p qs ps x0 x1 x2 base v1 v2 v3 ev lam sa [z0 z1 z2 zb zp] red
+//   RM_DENSE_GLOBAL  q p qs ps x0 x1 x2 base v1 v2 v3 ev red, panel buffers
+//   RM_MATRICES      [M1 M2 M3] q p qs ps x0 x1 x2 base v1 v2 v3 lam sa gsa ev Vn z0 z1 z2 zb zp
+//                    rc rs top bot red
+// where Vn and z0 .. zp take 2 dpad each, rc, rs and top / bot (ints) dpad / 2 + 2 each.
+__host__ __device__ __forceinline__ size_t rm_carve(const RmLayout& l, double* s, double* gmats,
+                                                    Blk& blk, RmWork& w, double** tscratch) {
+  double* const s0 = s;
+  const int dim = l.dim;
   const int ld = dim + 1;
   const int dpad = (dim + 1) & ~1;
   w.dim = dim;
   w.ld = ld;
-  if (n_mats == RM_NMATS_GLOBAL) {
+  size_t beyond = 0;  // doubles the policy carves from `extra` itself
+  if (l.place == RM_COMPACT) {
+    w.M1 = w.M2 = w.M3 = nullptr;
+    double** cv[] = {&w.q,  &w.p,  &w.qs, &w.ps, &w.x0, &w.x1, &w.x2,
+                     &w.base, &w.v1, &w.v2, &w.v3, &w.ev, &w.lam, &w.sa};
+    for (auto v : cv) {
+      *v = s;
+      s += dpad;
+    }
+    w.gsa = w.Vn = nullptr;
+    w.rc = w.rs = nullptr;
+    w.top = w.bot = nullptr;
+    if (l.zvecs) {
+      double** zv[] = {&w.z0, &w.z1, &w.z2, &w.zb, &w.zp};
+      for (auto v : zv) {
+        *v = s;
+        s += 2 * dpad;
+      }
+    } else {
+      w.z0 = w.z1 = w.z2 = w.zb = w.zp = nullptr;
+    }
+  } else if (l.place == RM_DENSE_GLOBAL) {
     w.M1 = w.M2 = w.M3 = nullptr;
     double** cv[] = {&w.q, &w.p, &w.qs, &w.ps, &w.x0, &w.x1, &w.x2, &w.base, &w.v1, &w.v2, &w.v3,
                      &w.ev};
@@ -429,114 +473,88 @@ __device__ inline void rm_carve(RmWork& w, double* s, int dim, int n_mats, Blk& 
     w.z0 = w.z1 = w.z2 = w.zb = w.zp = nullptr;
     w.rc = w.rs = nullptr;
     w.top = w.bot = nullptr;
-    blk.red = s;
-    s += 40;
-    w.extra = s;
-    return;
-  }
-  if (n_mats >= RM_NMATS_IN_WORKSPACE) {
-    const int km = n_mats - RM_NMATS_IN_WORKSPACE;
-    const size_t sq = ((size_t)dim * ld + 1) & ~(size_t)1;
-    w.M1 = km >= 1 ? gmats : nullptr;
-    w.M2 = km >= 2 ? gmats + sq : nullptr;
-    w.M3 = km >= 3 ? gmats + 2 * sq : nullptr;
-    n_mats = 0;
+    beyond = dg_smem_doubles(dim);
   } else {
-    w.M1 = n_mats >= 1 ? s : nullptr;
-    if (n_mats >= 1) s += (size_t)dim * ld;
-    w.M2 = n_mats >= 2 ? s : nullptr;
-    if (n_mats >= 2) s += (size_t)dim * ld;
-    w.M3 = n_mats >= 3 ? s : nullptr;
-    if (n_mats >= 3) s += (size_t)dim * ld;
-  }
-  double** vecs[] = {&w.q, &w.p, &w.qs, &w.ps, &w.x0, &w.x1, &w.x2, &w.base, &w.v1,
-                     &w.v2, &w.v3, &w.lam, &w.sa, &w.gsa, &w.ev};
-  for (auto v : vecs) {
-    *v = s;
-    s += dpad;
-  }
-  w.Vn = s;
-  s += 2 * dpad;
-  w.z0 = s;
-  s += 2 * dpad;
-  w.z1 = s;
-  s += 2 * dpad;
-  w.z2 = s;
-  s += 2 * dpad;
-  w.zb = s;
-  s += 2 * dpad;
-  w.zp = s;
-  s += 2 * dpad;
-  w.rc = s;
-  s += dpad / 2 + 2;
-  w.rs = s;
-  s += dpad / 2 + 2;
-  w.top = reinterpret_cast<int*>(s);
-  w.bot = w.top + (dpad / 2 + 2);
-  s += dpad / 2 + 2;
-  blk.red = s;
-  w.extra = s + 40;
-}
-
-// Compact vector set of the O(D) metric policies (COMPACT: diagonal and scalar metrics): the
-// integrator's vectors q p qs ps x0 x1 x2 base v1 v2 v3 plus ev (policy scratch), lam (d(q)) and
-// sa (1 / d(q)); the implicit-midpoint vectors z0 z1 z2 zb zp [2 dpad each] only when `midpoint`
-// is set.  No matrices, no eigensolver or Cholesky buffers: at D = 128 a chain needs 14.6 KB
-// (leapfrog), so that many chains share an SM.
-__host__ __device__ inline size_t rm_compact_doubles(int dim, int midpoint) {
-  const int dpad = (dim + 1) & ~1;
-  return (size_t)(midpoint ? 24 : 14) * dpad + 40;
-}
-
-__device__ inline void rm_carve_compact(RmWork& w, double* s, int dim, int midpoint, Blk& blk) {
-  const int dpad = (dim + 1) & ~1;
-  w.dim = dim;
-  w.ld = dim + 1;
-  w.M1 = w.M2 = w.M3 = nullptr;
-  double** cv[] = {&w.q,  &w.p,  &w.qs, &w.ps, &w.x0, &w.x1, &w.x2,
-                   &w.base, &w.v1, &w.v2, &w.v3, &w.ev, &w.lam, &w.sa};
-  for (auto v : cv) {
-    *v = s;
-    s += dpad;
-  }
-  w.gsa = w.Vn = nullptr;
-  w.rc = w.rs = nullptr;
-  w.top = w.bot = nullptr;
-  if (midpoint) {
-    double** zv[] = {&w.z0, &w.z1, &w.z2, &w.zb, &w.zp};
-    for (auto v : zv) {
-      *v = s;
-      s += 2 * dpad;
+    if (l.ws_mats > 0) {
+      const int km = l.ws_mats;
+      const size_t sq = l.ws_mat_doubles();
+      w.M1 = km >= 1 ? gmats : nullptr;
+      w.M2 = km >= 2 ? gmats + sq : nullptr;
+      w.M3 = km >= 3 ? gmats + 2 * sq : nullptr;
+    } else {
+      const int nm = l.smem_mats;
+      w.M1 = nm >= 1 ? s : nullptr;
+      if (nm >= 1) s += (size_t)dim * ld;
+      w.M2 = nm >= 2 ? s : nullptr;
+      if (nm >= 2) s += (size_t)dim * ld;
+      w.M3 = nm >= 3 ? s : nullptr;
+      if (nm >= 3) s += (size_t)dim * ld;
     }
-  } else {
-    w.z0 = w.z1 = w.z2 = w.zb = w.zp = nullptr;
+    double** vecs[] = {&w.q, &w.p, &w.qs, &w.ps, &w.x0, &w.x1, &w.x2, &w.base, &w.v1,
+                       &w.v2, &w.v3, &w.lam, &w.sa, &w.gsa, &w.ev};
+    for (auto v : vecs) {
+      *v = s;
+      s += dpad;
+    }
+    w.Vn = s;  // NEED <= 2 entries per coordinate
+    s += 2 * dpad;
+    w.z0 = s;
+    s += 2 * dpad;
+    w.z1 = s;
+    s += 2 * dpad;
+    w.z2 = s;
+    s += 2 * dpad;
+    w.zb = s;
+    s += 2 * dpad;
+    w.zp = s;
+    s += 2 * dpad;
+    w.rc = s;
+    s += dpad / 2 + 2;
+    w.rs = s;
+    s += dpad / 2 + 2;
+    w.top = reinterpret_cast<int*>(s);
+    w.bot = w.top + (dpad / 2 + 2);
+    s += dpad / 2 + 2;
   }
   blk.red = s;
-  w.extra = s + 40;
+  s += 40;
+  w.extra = s;
+  // DENSE_MTP targets (SoftAbs, RM_THREADS): the per-warp staging rows and the per-direction
+  // results take (nwarp + 1) x dim doubles of the Vn / z0 .. zp region, which is contiguous, and
+  // this scratch the next dim: the region's 12 dpad hold (nwarp + 2) x dim
+  static_assert(RM_THREADS / 32 + 2 <= 12, "DENSE_MTP scratch beyond the Vn / z region");
+  *tscratch = w.Vn != nullptr ? w.Vn + (size_t)(blk.nwarp + 1) * dim : nullptr;
+  return (size_t)(s - s0) + beyond;
 }
 
-// true for metric policies that declare `static constexpr bool COMPACT = true` (carved by
-// rm_carve_compact); the matrix policies declare nothing and keep rm_carve
-template <class M, class = void>
-struct rm_compact_policy {
-  static constexpr bool value = false;
-};
-template <class M>
-struct rm_compact_policy<M, decltype(void(M::COMPACT))> {
-  static constexpr bool value = M::COMPACT;
-};
+__host__ __device__ inline size_t rm_smem_bytes(const RmLayout& l) {
+  Blk blk{};
+  RmWork w;
+  double* tscratch;
+  return rm_carve(l, nullptr, nullptr, blk, w, &tscratch) * sizeof(double);
+}
 
-// number of per-chain D x D matrices a policy keeps in the per-CTA global workspace
-// (n_mats = RM_NMATS_IN_WORKSPACE + value) when its shared-memory layout does not fit: policies
-// that declare `static constexpr int WORKSPACE_MATS`; 0 (no such route) for the others
-template <class M, class = void>
-struct rm_workspace_mats {
-  static constexpr int value = 0;
-};
-template <class M>
-struct rm_workspace_mats<M, decltype(void(M::WORKSPACE_MATS))> {
-  static constexpr int value = M::WORKSPACE_MATS;
-};
+// The start of every Riemannian kernel: the CTA's Blk, and the chain's buffers carved by layout
+// `l` from dynamic shared memory and this CTA's share of m.workspace.  Returns the scratch of
+// DENSE_MTP targets (Target::attach).  COMPACT: the kernel's policy is an RM_COMPACT one, so
+// every layout it is launched with is; a matrix policy's kernel is never launched with one.
+// STEPS: the kernel integrates (the velocity and momentum kernels take no step, so a compact
+// layout carves no midpoint vectors for them).  Stating both at compile time leaves only the
+// carves that can run in the kernel.
+template <bool COMPACT, bool STEPS = true>
+__device__ __forceinline__ double* rm_begin(RmLayout l, const ModelArgs& m, Blk& blk,
+                                            RmWork& w) {
+  extern __shared__ double smem[];
+  blk.tid = threadIdx.x, blk.nthr = blockDim.x, blk.lane = threadIdx.x & 31;
+  blk.warp = threadIdx.x >> 5, blk.nwarp = blockDim.x >> 5;
+  l.place = COMPACT ? RM_COMPACT : l.place == RM_DENSE_GLOBAL ? RM_DENSE_GLOBAL : RM_MATRICES;
+  if (!STEPS) l.zvecs = false;
+  double* tscratch;
+  rm_carve(l, smem,
+           m.workspace != nullptr ? m.workspace + (size_t)blockIdx.x * m.ws_stride : nullptr, blk,
+           w, &tscratch);
+  return tscratch;
+}
 
 // true for policies whose build() accepts a metric that cannot be solved with (a zero pivot of
 // a triangular factor: `static constexpr bool CAN_BE_SINGULAR = true` and a `singular()`
@@ -865,6 +883,11 @@ __device__ inline void smem_matmul(const Blk& k, int n, int ld, const double* X,
 }
 
 #ifndef __CUDACC_RTC__  // library self-tests: kept out of the run-time compiled user images
+// three matrices in shared memory: the eigenvectors, the matrix, and the warm start's product
+__host__ __device__ inline RmLayout eigh_selftest_layout(int dim) {
+  return RmLayout{dim, RM_MATRICES, 3, 0, true};
+}
+
 // Diagnostic kernel: K3 on arbitrary dense symmetric matrices (one CTA per matrix).  With
 // `warm_from` >= 0 the solve of matrix i is warm-started from the eigenvectors of matrix
 // `warm_from` (exercising the V^T H V path used between fixed-point iterates).
@@ -877,7 +900,8 @@ static __global__ void __launch_bounds__(RM_THREADS)
   blk.tid = threadIdx.x, blk.nthr = blockDim.x, blk.lane = threadIdx.x & 31;
   blk.warp = threadIdx.x >> 5, blk.nwarp = blockDim.x >> 5;
   RmWork w;
-  rm_carve(w, smem, dim, 3, blk);
+  double* tscratch;
+  rm_carve(eigh_selftest_layout(dim), smem, nullptr, blk, w, &tscratch);
   const int ld = w.ld;
   for (int64_t mi = blockIdx.x; mi < n_mats; mi += gridDim.x) {
     __syncthreads();
@@ -986,6 +1010,7 @@ __device__ inline void cholesky_solve(const Blk& k, const double* L, int n, int 
 template <class Target>
 struct SoftAbsMetric {
   static constexpr bool SOFTABS = true;
+  static constexpr RmPlace PLACE = RM_MATRICES;
   static constexpr int N_MATS = 2;
   // beyond shared memory: eigenvectors, work / divided-difference and warm-start matrices
   static constexpr int WORKSPACE_MATS = 3;
@@ -1243,7 +1268,9 @@ struct SoftAbsMetric {
 template <class Target>
 struct Rank1DenseMetric {
   static constexpr bool SOFTABS = false;
+  static constexpr RmPlace PLACE = RM_MATRICES;
   static constexpr int N_MATS = 1;
+  static constexpr int WORKSPACE_MATS = 0;
   static constexpr int MIN_BLOCKS = 2;
   static constexpr int THREADS = RM_THREADS;
   const Target& t;
@@ -1315,7 +1342,9 @@ struct Rank1DenseMetric {
 template <class Target>
 struct Rank1WoodburyMetric {
   static constexpr bool SOFTABS = false;
+  static constexpr RmPlace PLACE = RM_MATRICES;
   static constexpr int N_MATS = 0;
+  static constexpr int WORKSPACE_MATS = 0;
   static constexpr int MIN_BLOCKS = 2;
   static constexpr int THREADS = RM_THREADS;
   const Target& t;
@@ -1432,8 +1461,9 @@ struct FunnelFisherDiagModel {
 template <class Target, class Model>
 struct DiagonalMetric {
   static constexpr bool SOFTABS = false;
-  static constexpr bool COMPACT = true;
+  static constexpr RmPlace PLACE = RM_COMPACT;
   static constexpr int N_MATS = 0;
+  static constexpr int WORKSPACE_MATS = 0;
   static constexpr int MIN_BLOCKS = RM_COMPACT_MIN_BLOCKS;
   static constexpr int THREADS = RM_COMPACT_THREADS;
   const Target& t;
@@ -1513,8 +1543,9 @@ struct QuadraticScalarModel {
 template <class Target, class Model>
 struct ScalarMetric {
   static constexpr bool SOFTABS = false;
-  static constexpr bool COMPACT = true;
+  static constexpr RmPlace PLACE = RM_COMPACT;
   static constexpr int N_MATS = 0;
+  static constexpr int WORKSPACE_MATS = 0;
   static constexpr int MIN_BLOCKS = RM_COMPACT_MIN_BLOCKS;
   static constexpr int THREADS = RM_COMPACT_THREADS;
   const Target& t;
@@ -1564,19 +1595,10 @@ struct ScalarMetric {
 template <class Target>
 using QuadraticScalarMetric = ScalarMetric<Target, QuadraticScalarModel>;
 
-// What the host's launch plan (rm_launch) reads of a user image's policies, DiagonalMetric and
-// ScalarMetric over the user functions of user_riemannian.cuh: that header, which NVRTC compiles,
-// checks that its policies carry these values.
+// What the host's launch plan (rm_launch) reads of a user image's target (UserRTarget of
+// user_riemannian.cuh derives from it); the image's policies are the registry's, over user models
 struct UserRTargetTraits {
   static constexpr bool DENSE_MTP = false;
-};
-template <class>
-struct UserRPolicyTraits {
-  static constexpr bool SOFTABS = false;
-  static constexpr bool COMPACT = true;
-  static constexpr int N_MATS = 0;
-  static constexpr int MIN_BLOCKS = RM_COMPACT_MIN_BLOCKS;
-  static constexpr int THREADS = RM_COMPACT_THREADS;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -1683,6 +1705,7 @@ template <class Target, class Model>
 struct CholeskyFactoredMetric {
   static constexpr bool SOFTABS = false;
   static constexpr bool CAN_BE_SINGULAR = true;
+  static constexpr RmPlace PLACE = RM_MATRICES;
   // the factor [dim x (dim + 1)], and V for a DENSE_VJP model; in the per-CTA global workspace
   // beyond D ~ 150 (one matrix) or D ~ 113 (two)
   static constexpr int N_MATS = chol_dense_vjp<Model>::value ? 2 : 1;
@@ -1766,16 +1789,11 @@ struct CholeskyFactoredMetric {
 template <class Target>
 using QuadraticCholeskyMetric = CholeskyFactoredMetric<Target, QuadraticCholModel>;
 
-// What rm_launch reads of a user image's Cholesky-factored policy (CholeskyFactoredMetric over the
-// user functions of user_riemannian.cuh, which checks these values): the factor and V per chain
-template <class>
-struct UserRCholPolicyTraits {
-  static constexpr bool SOFTABS = false;
-  static constexpr bool COMPACT = false;
-  static constexpr int N_MATS = 2;
-  static constexpr int WORKSPACE_MATS = 2;
-  static constexpr int MIN_BLOCKS = 1;
-  static constexpr int THREADS = MB200_RM_CHOL_THREADS;
+// What rm_launch reads of the model of a user image's Cholesky-factored policy (UserCholModel of
+// user_riemannian.cuh derives from it): CholeskyFactoredMetric<UserRTargetTraits,
+// UserCholModelTraits> carries the image policy's launch constants
+struct UserCholModelTraits {
+  static constexpr bool DENSE_VJP = true;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -2130,24 +2148,12 @@ __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN
                              double fp_div, int fp_max, double rev_tol,
                              double* __restrict__ h_out, int32_t* __restrict__ status,
                              int32_t* __restrict__ n_done, int32_t* __restrict__ fp_iters,
-                             int n_mats, int midpoint, int fp_solver) {
-  extern __shared__ double smem[];
+                             RmLayout layout, int midpoint, int fp_solver) {
   Blk blk;
-  blk.tid = threadIdx.x;
-  blk.nthr = blockDim.x;
-  blk.lane = threadIdx.x & 31;
-  blk.warp = threadIdx.x >> 5;
-  blk.nwarp = blockDim.x >> 5;
   RmWork w;
-  if constexpr (rm_compact_policy<MetricT<Target>>::value)
-    rm_carve_compact(w, smem, dim, midpoint, blk);
-  else
-    rm_carve(w, smem, dim, n_mats, blk,
-             model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
-                                        : nullptr);
+  double* const tscratch = rm_begin<MetricT<Target>::PLACE == RM_COMPACT>(layout, model, blk, w);
   const Target target(model, dim);
-  // scratch of DENSE_MTP targets: [dim] doubles behind the staging rows in the Vn / z region
-  target.attach(w.Vn != nullptr ? w.Vn + (size_t)(blk.nwarp + 1) * dim : nullptr);
+  target.attach(tscratch);
   MetricT<Target> metric(target, model);
   ImplicitLeapfrog<Target, MetricT<Target>> integ{blk,    w,      target,  metric,
                                                   fp_tol, fp_div, rev_tol, fp_max, fp_solver};
@@ -2208,21 +2214,14 @@ template <class Target, template <class> class MetricT>
 __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN_BLOCKS)
     riemannian_sample_momentum_kernel(const double* __restrict__ q_in, const double* __restrict__ z,
                                       double* __restrict__ p_out, int64_t n_chains, int dim,
-                                      ModelArgs model, int32_t* __restrict__ status, int n_mats) {
-  extern __shared__ double smem[];
+                                      ModelArgs model, int32_t* __restrict__ status,
+                                      RmLayout layout) {
   Blk blk;
-  blk.tid = threadIdx.x, blk.nthr = blockDim.x, blk.lane = threadIdx.x & 31;
-  blk.warp = threadIdx.x >> 5, blk.nwarp = blockDim.x >> 5;
   RmWork w;
-  if constexpr (rm_compact_policy<MetricT<Target>>::value)
-    rm_carve_compact(w, smem, dim, 0, blk);
-  else
-    rm_carve(w, smem, dim, n_mats, blk,
-             model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
-                                        : nullptr);
+  double* const tscratch =
+      rm_begin<MetricT<Target>::PLACE == RM_COMPACT, false>(layout, model, blk, w);
   const Target target(model, dim);
-  // scratch of DENSE_MTP targets: [dim] doubles behind the staging rows in the Vn / z region
-  target.attach(w.Vn != nullptr ? w.Vn + (size_t)(blk.nwarp + 1) * dim : nullptr);
+  target.attach(tscratch);
   MetricT<Target> metric(target, model);
   for (int64_t ch = blockIdx.x; ch < n_chains; ch += gridDim.x) {
     __syncthreads();
@@ -2246,21 +2245,14 @@ template <class Target, template <class> class MetricT>
 __global__ void __launch_bounds__(MetricT<Target>::THREADS, MetricT<Target>::MIN_BLOCKS)
     riemannian_velocity_kernel(const double* __restrict__ q_in, const double* __restrict__ p_in,
                                double* __restrict__ vel_out, int64_t n_chains, int dim,
-                               ModelArgs model, int32_t* __restrict__ status, int n_mats) {
-  extern __shared__ double smem[];
+                               ModelArgs model, int32_t* __restrict__ status,
+                                      RmLayout layout) {
   Blk blk;
-  blk.tid = threadIdx.x, blk.nthr = blockDim.x, blk.lane = threadIdx.x & 31;
-  blk.warp = threadIdx.x >> 5, blk.nwarp = blockDim.x >> 5;
   RmWork w;
-  if constexpr (rm_compact_policy<MetricT<Target>>::value)
-    rm_carve_compact(w, smem, dim, 0, blk);
-  else
-    rm_carve(w, smem, dim, n_mats, blk,
-             model.workspace != nullptr ? model.workspace + (size_t)blockIdx.x * model.ws_stride
-                                        : nullptr);
+  double* const tscratch =
+      rm_begin<MetricT<Target>::PLACE == RM_COMPACT, false>(layout, model, blk, w);
   const Target target(model, dim);
-  // scratch of DENSE_MTP targets: [dim] doubles behind the staging rows in the Vn / z region
-  target.attach(w.Vn != nullptr ? w.Vn + (size_t)(blk.nwarp + 1) * dim : nullptr);
+  target.attach(tscratch);
   MetricT<Target> metric(target, model);
   for (int64_t ch = blockIdx.x; ch < n_chains; ch += gridDim.x) {
     __syncthreads();

@@ -87,8 +87,7 @@ static_assert(RM_COMPACT_THREADS == 32, "the user contract is per warp: one chai
 
 // Riemannian block interface (riemannian.cuh) over the user's target functions: l and grad l
 // only, no Hessian
-struct UserRTarget {
-  static constexpr bool DENSE_MTP = false;
+struct UserRTarget : UserRTargetTraits {
   static constexpr bool HAS_HESSIAN = false;
   static constexpr int NEED = 1;
   UserTarget u;  // target_params and target_aux
@@ -110,7 +109,6 @@ struct UserRTarget {
   __device__ __forceinline__ int need_col(int, int) const { return -1; }
   __device__ void mtp_entries(const Blk&, const double*, const double*, double*) const {}
 };
-static_assert(UserRTarget::DENSE_MTP == UserRTargetTraits::DENSE_MTP, "host launch traits");
 
 // The metric's view of a chain: rmetric_params and rmetric_aux
 struct UserMetricArgs {
@@ -237,8 +235,7 @@ struct UserCtaMetricArgs {
 // policy's own finiteness check of the lower triangle (the user function returns nothing), and
 // the VJP of a lower-triangular V (DENSE_VJP: the policy forms V in w.M2)
 template <class F = UserMetricFunctions>
-struct UserCholModel : UserCtaMetricArgs {
-  static constexpr bool DENSE_VJP = true;
+struct UserCholModel : UserCtaMetricArgs, UserCholModelTraits {
   __device__ UserCholModel(const ModelArgs& m, int d) : UserCtaMetricArgs(m, d) {}
   // true iff every entry of the lower triangle is finite
   __device__ bool fill(const Blk& k, const double* q, double* L, int ld) const {
@@ -304,25 +301,6 @@ template <class Target>
 using UserDenseMetric = GlobalDenseMetricT<Target, UserDenseModel<>>;
 static_assert(DG_THREADS == 256, "the dense user contract is per 256-thread CTA");
 #endif
-
-template <class P>
-constexpr bool user_policy_traits_match() {
-  using H = UserRPolicyTraits<UserRTarget>;
-  return P::SOFTABS == H::SOFTABS && P::COMPACT == H::COMPACT && P::N_MATS == H::N_MATS &&
-         P::MIN_BLOCKS == H::MIN_BLOCKS && P::THREADS == H::THREADS;
-}
-static_assert(user_policy_traits_match<DiagonalMetric<UserRTarget, QuadraticDiagModel>>() &&
-                  user_policy_traits_match<ScalarMetric<UserRTarget, QuadraticScalarModel>>(),
-              "host launch traits");
-
-template <class P>
-constexpr bool user_chol_traits_match() {
-  using H = UserRCholPolicyTraits<UserRTargetCta>;
-  return P::SOFTABS == H::SOFTABS && rm_compact_policy<P>::value == H::COMPACT &&
-         P::N_MATS == H::N_MATS && rm_workspace_mats<P>::value == H::WORKSPACE_MATS &&
-         P::MIN_BLOCKS == H::MIN_BLOCKS && P::THREADS == H::THREADS;
-}
-static_assert(user_chol_traits_match<UserCholeskyMetric<UserRTargetCta>>(), "host launch traits");
 
 }  // namespace mb200
 

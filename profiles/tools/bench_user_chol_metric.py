@@ -59,11 +59,15 @@ def compile_and_load(system):
     return time.perf_counter() - t0
 
 
+RM_SMEM_BYTES = 227 * 1024  # riemannian.cuh: opt-in shared memory per CTA on sm_90
+
+
 def layout(dim, n_mats):
-    """Where the launch plan keeps a chain's matrices (riemannian.cuh rm_smem_doubles)."""
+    """Where the launch plan keeps a chain's matrices: the size rm_carve (riemannian.cuh) gives an
+    RM_MATRICES layout with n_mats matrices, against RM_SMEM_BYTES."""
     ld, dpad = dim + 1, (dim + 1) & ~1
     vec = 27 * dpad + 3 * (dpad // 2 + 2) + 40
-    return "shared" if (dim * ld * n_mats + vec) * 8 <= 227 * 1024 else "workspace"
+    return "shared" if (dim * ld * n_mats + vec) * 8 <= RM_SMEM_BYTES else "workspace"
 
 
 def main():
